@@ -8,6 +8,7 @@ from __future__ import annotations
 import os
 import subprocess
 import sys
+import tempfile
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
@@ -88,9 +89,16 @@ def build_mirror(force: bool = False) -> Path:
 
 
 def build_cpp_program(src: Path, out: Path) -> Path:
-    """compile + link a C++ program against the mirror (used by tests/test_cpp_mirror.py)"""
+    """compile + link a C++ program against the mirror (used by tests/test_cpp_mirror.py); returns the executable, which is `out`
+    or, when the tree cannot be written (a checkout owned by another user), a file of the same name in a fresh temporary directory"""
     build_mirror()
-    out.parent.mkdir(parents=True, exist_ok=True)
+    try:
+        out.parent.mkdir(parents=True, exist_ok=True)
+        writable = os.access(out.parent, os.W_OK)
+    except OSError:
+        writable = False
+    if not writable:
+        out = Path(tempfile.mkdtemp(prefix="dfusion_cpp_")) / out.name
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     cmd = [nvcc, "-std=c++17", "-O1", *MIRROR_INC, "-o", str(out), str(src), "-L", str(HERE), "-lkfusion", "-ldfusion",
            "-Xlinker", "-rpath", "-Xlinker", str(HERE)]

@@ -9,7 +9,6 @@
 //                          double-precision warp-shuffle reduction and one partial row per block (deterministic order);
 //   icp_solve_kernel       one block: fixed-order sum of the partials, 6x6 solve, Rodrigues, T <- Tinc * T in place.
 #include "df_common.cuh"
-#include <cstring>
 #include <float.h>
 #include <stdlib.h>
 
@@ -304,8 +303,8 @@ __device__ void sym6_solve_dev(const double *Ain, const double *b, double *x)
 }
 
 // host step projective_icp.cpp:195-209 on the device: sums -> A, b -> r = solve(A, b) -> T <- Affine3f(r) * T.  Tin/Tout: 12 floats
-// (R row-major, t).  Returns false where the reference returns false (|det| < 1e-15 or NaN).  `r` solved by the caller-provided
-// Cholesky (chol6_solve in registers, or the warp version below); this part is the general fallback + the pose composition.
+// (R row-major, t).  Returns false where the reference returns false (|det| < 1e-15 or NaN).  `r` solved by the caller's
+// Cholesky (chol6_solve, in registers); this part is the general fallback + the pose composition.
 __device__ bool icp_fallback_solve(const double (&A)[36], const double (&b)[6], double (&r)[6])
 {
     const double det = det6_dev(A);
@@ -343,27 +342,6 @@ __device__ void icp_compose_pose(const double (&r)[6], const float *Tin, float *
     for (int i = 0; i < 3; ++i) Tout[9 + i] = tn[i];
 }
 
-// out-of-line versions over shared memory for the persistent kernel (keeps the register needs of these one-thread tails away from
-// its 768-thread accumulate loop)
-__device__ __noinline__ bool icp_fallback_smem(const double *sA, const double *sb, double *sr)
-{
-    double A[36], b[6], r[6];
-    for (int i = 0; i < 36; ++i) A[i] = sA[i];
-    for (int i = 0; i < 6; ++i) b[i] = sb[i];
-    if (!icp_fallback_solve(A, b, r)) return false;
-    for (int i = 0; i < 6; ++i) sr[i] = r[i];
-    return true;
-}
-__device__ __noinline__ void icp_compose_pose_smem(const double *sr, float *Ts)
-{
-    double r[6];
-    float Tin[12], Tn[12];
-    for (int i = 0; i < 6; ++i) r[i] = sr[i];
-    for (int i = 0; i < 12; ++i) Tin[i] = Ts[i];
-    icp_compose_pose(r, Tin, Tn);
-    for (int i = 0; i < 12; ++i) Ts[i] = Tn[i];
-}
-
 // A (symmetric) and b from the 27 sums; the reference's buffer is float (projective_icp.cpp:51-60)
 __device__ __forceinline__ void icp_unpack_sums(const double *sums, double (&A)[36], double (&b)[6])
 {
@@ -399,272 +377,6 @@ __global__ void __launch_bounds__(256) icp_solve_kernel(const double *partials, 
         if (!icp_fallback_solve(A, b, r)) { *ok = 0; return; }
     } else if (fabs(det) < 1e-15 || det != det) { *ok = 0; return; }     // projective_icp.cpp:197-203
     icp_compose_pose(r, Tin, T);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// The whole coarse-to-fine loop (19 iterations at the default 4 + 5 + 10) as ONE persistent launch: one CTA per SM, a grid barrier
-// per iteration.  Round 1 ran 19 x (accumulate, solve) = 38 dependent launches, each paying its launch latency.  Here every
-// CTA accumulates its share of the level's pixels, publishes its 27 partial sums (double-buffered by iteration parity), waits at
-// the barrier, then EVERY CTA sums the partials in the same fixed order and solves the same 6 x 6 system -- identical arithmetic on
-// identical data, so all CTAs hold bit-identical poses and nobody has to broadcast one: a single barrier per iteration.
-// The 6 x 6 Cholesky runs on the lanes of warp 0 over shared memory (row i on lane i): the accumulate loop's register budget
-// (768 threads) is not touched by the solve, which is what made the fused last-block tail of round 1 lose.
-struct IcpLevelView {
-    const float4 *vcurr, *ncurr, *vprev, *nprev;
-    const unsigned short *dcurr, *dprev;
-    size_t pitch, dpitch;
-    int cols, rows, iters;
-    float fx, fy, cx, cy;
-};
-struct IcpPersistParams {
-    IcpLevelView lv[4];
-    int levels;
-    float dist2_thres, min_cosine;
-    double *partials;          // [2][gridDim.x][27]
-    unsigned int *barrier;     // [0] arrivals (monotone within a launch), [1] exits; both zero between launches
-    float *T_out; int *ok_out;
-};
-
-__device__ __forceinline__ void icp_grid_barrier(unsigned int *counter, unsigned int target)
-{
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(counter, 1u);
-        unsigned int v;
-        do { asm volatile("ld.acquire.gpu.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory"); } while (v < target);
-    }
-    __syncthreads();
-}
-
-// warp 0: solve A r = b by Cholesky over shared memory; returns (in every lane of warp 0) 1 = ok, 0 = reference returns false,
-// 2 = not safely positive definite (caller takes the general path).  Same tests as chol6_solve.
-__device__ __noinline__ int chol6_warp(double *A, double *bvec, double *L, double *rout)
-{
-    const int lane = threadIdx.x & 31;
-    const unsigned full = 0xffffffffu;
-    double dmax = 0.0;
-    for (int i = 0; i < 6; ++i) dmax = fmax(dmax, fabs(A[i * 6 + i]));
-    bool ok = true;
-    double dprod = 1.0;
-    for (int j = 0; j < 6; ++j) {
-        double s = 0.0;
-        if (lane >= j && lane < 6) {
-            s = A[lane * 6 + j];
-            for (int k = 0; k < j; ++k) s -= L[lane * 6 + k] * L[j * 6 + k];
-        }
-        double d = __shfl_sync(full, s, j);
-        if (!(d > dmax * 1e-13)) { ok = false; d = 1.0; }
-        d = sqrt(d);
-        dprod *= d;
-        if (lane == j) L[j * 6 + j] = d;
-        else if (lane > j && lane < 6) L[lane * 6 + j] = s * (1.0 / d);
-        __syncwarp();
-    }
-    // forward: y_i = (b_i - sum_{k<i} L_ik y_k) / L_ii ; lanes keep their own running b
-    double bi = lane < 6 ? bvec[lane] : 0.0;
-    double yi = 0.0;
-    for (int i = 0; i < 6; ++i) {
-        const double y = __shfl_sync(full, bi, i) / L[i * 6 + i];
-        if (lane == i) yi = y;
-        if (lane > i && lane < 6) bi -= L[lane * 6 + i] * y;
-    }
-    // backward: x_i = (y_i - sum_{k>i} L_ki x_k) / L_ii
-    double xi = 0.0;
-    for (int i = 5; i >= 0; --i) {
-        const double x = __shfl_sync(full, yi, i) / L[i * 6 + i];
-        if (lane == i) xi = x;
-        if (lane < i) yi -= L[i * 6 + lane] * x;
-    }
-    if (lane < 6) rout[lane] = xi;
-    __syncwarp();
-    const double det = dprod * dprod;
-    if (!ok) return 2;
-    return (fabs(det) < 1e-15 || det != det) ? 0 : 1;
-}
-
-template <bool DEPTH, int NT>
-__global__ void __launch_bounds__(NT, 1) icp_persistent_kernel(const IcpPersistParams q)
-{
-    constexpr int NW = NT / 32;
-    __shared__ double smem[NW][27];
-    __shared__ double sums[27];
-    __shared__ __align__(16) double stage[RED_ROWS * 27];
-    __shared__ double sA[36], sL[36], sb[6], sr[6];
-    __shared__ float Ts[12];
-    __shared__ int ok_s;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    pdl_wait();
-    pdl_trigger();
-    if (tid < 12) Ts[tid] = (tid < 9 && tid % 4 == 0) ? 1.f : 0.f;      // affine = Identity, projective_icp.cpp:175
-    if (tid == 0) ok_s = 1;
-    __syncthreads();
-    unsigned int arrivals = 0;
-    int parity = 0;
-    for (int level = q.levels - 1; level >= 0 && ok_s; --level) {
-        const IcpLevelView &lv = q.lv[level];
-        IcpParams p;
-        p.vcurr = lv.vcurr; p.ncurr = lv.ncurr; p.vprev = lv.vprev; p.nprev = lv.nprev;
-        p.vcpitch = p.ncpitch = p.vppitch = p.nppitch = lv.pitch;
-        p.dcurr = lv.dcurr; p.dprev = lv.dprev; p.dcpitch = p.dppitch = lv.dpitch;
-        p.cols = lv.cols; p.rows = lv.rows; p.fcols = (float)lv.cols; p.frows = (float)lv.rows;
-        p.fx = lv.fx; p.fy = lv.fy; p.cx = lv.cx; p.cy = lv.cy; p.finvx = 1.f / lv.fx; p.finvy = 1.f / lv.fy;
-        p.dist2_thres = q.dist2_thres; p.min_cosine = q.min_cosine;
-        const int npix = lv.cols * lv.rows;
-        for (int it = 0; it < lv.iters && ok_s; ++it) {
-            Aff T;
-            T.r0 = make_float3(Ts[0], Ts[1], Ts[2]); T.r1 = make_float3(Ts[3], Ts[4], Ts[5]); T.r2 = make_float3(Ts[6], Ts[7], Ts[8]);
-            T.t = make_float3(Ts[9], Ts[10], Ts[11]);
-            float acc[27];
-#pragma unroll
-            for (int i = 0; i < 27; ++i) acc[i] = 0.f;
-            for (int i = blockIdx.x * NT + tid; i < npix; i += gridDim.x * NT) {
-                const int y = i / lv.cols, x = i - y * lv.cols;
-                float row[7];
-                if (icp_row<DEPTH>(p, T, x, y, row)) {
-                    int k = 0;
-#pragma unroll
-                    for (int a = 0; a < 6; ++a)
-#pragma unroll
-                        for (int j = a; j < 7; ++j) acc[k++] += row[a] * row[j];
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 27; ++i) {
-                float v = acc[i];                                   // float warp stage, see icp_accumulate_kernel
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-                if (lane == 0) smem[warp][i] = (double)v;
-            }
-            __syncthreads();
-            double *mine = q.partials + ((size_t)parity * gridDim.x + blockIdx.x) * 27;
-            if (tid < 27) {
-                double v = 0.0;
-#pragma unroll
-                for (int w = 0; w < NW; ++w) v += smem[w][tid];
-                mine[tid] = v;
-            }
-            arrivals += gridDim.x;
-            icp_grid_barrier(q.barrier, arrivals);
-            reduce_partials(q.partials + (size_t)parity * gridDim.x * 27, gridDim.x, sums, stage);
-            if (warp == 0) {
-                if (lane == 0) {                                        // A (symmetric), b from the 27 sums; the reference's buffer is float
-                    int shift = 0;
-                    for (int i = 0; i < 6; ++i)
-                        for (int j = i; j < 7; ++j) {
-                            const double value = (double)(float)sums[shift++];
-                            if (j == 6) sb[i] = value; else sA[j * 6 + i] = sA[i * 6 + j] = value;
-                        }
-                }
-                __syncwarp();
-                const int st = chol6_warp(sA, sb, sL, sr);
-                if (lane == 0) {
-                    bool good = st == 1;
-                    if (st == 2) good = icp_fallback_smem(sA, sb, sr);  // not safely SPD (or NaN): the general path of icp_solve_kernel
-                    if (good) icp_compose_pose_smem(sr, Ts);
-                    else ok_s = 0;
-                }
-            }
-            __syncthreads();
-            parity ^= 1;
-        }
-    }
-    if (blockIdx.x == 0 && tid < 12) q.T_out[tid] = Ts[tid];
-    if (blockIdx.x == 0 && tid == 0) *q.ok_out = ok_s;
-    if (tid == 0) {                                                     // the last CTA out leaves the barrier words zero for the next launch
-        __threadfence();
-        const unsigned int gone = atomicAdd(q.barrier + 1, 1u);
-        if (gone == gridDim.x - 1) { q.barrier[0] = 0u; q.barrier[1] = 0u; __threadfence(); }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Chained variant (round 2, second session; DF_ICP_CHAINED=1, measured and kept opt-in): one launch per ITERATION instead of two.  Every CTA of iteration
-// k first sums the partials of iteration k-1 in the fixed order and solves the same 6 x 6 system on the lanes of warp 0 (the persistent
-// kernel's code: identical arithmetic on identical data in every CTA, nobody broadcasts a pose), then accumulates with the new pose.  What
-// the persistent kernel paid a grid barrier for is a programmatic-dependent-launch boundary here, and the 19 separate solve launches of the
-// two-kernel chain are gone: 19 + 1 launches instead of 38.  Pose, gate and partials are double-buffered by iteration parity (block 0
-// publishes the pose the others are still reading the old copy of).  Measured slower than the
-// two-kernel chain -- the same verdict as for the persistent kernel: with the solve as every CTA's prologue its serial latency (plus the
-// SM-count-way redundant reduction) sits in front of all the accumulate blocks, while the one-block solve kernel overlaps its launch with the
-// accumulate blocks' drain.  A launch boundary saved is worth less than that.
-template <bool DEPTH, int NT>
-__global__ void __launch_bounds__(NT, 1) icp_chain_kernel(const IcpParams p, const double *prev_partials, int prev_blocks, const float *T_in, const int *ok_in,
-                                                       float *T_out, int *ok_out)
-{
-    constexpr int NW = NT / 32;
-    __shared__ double smem[NW][27];
-    __shared__ double sums[27];
-    __shared__ __align__(16) double stage[RED_ROWS * 27];
-    __shared__ double sA[36], sL[36], sb[6], sr[6];
-    __shared__ float Ts[12];
-    __shared__ int ok_s;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    pdl_wait();
-    pdl_trigger();
-    if (tid < 12) Ts[tid] = T_in[tid];
-    if (tid == 0) ok_s = *ok_in;
-    __syncthreads();
-    if (prev_blocks > 0 && ok_s) {                                       // the solve of the previous iteration (block-uniform condition)
-        reduce_partials(prev_partials, prev_blocks, sums, stage);
-        if (warp == 0) {
-            if (lane == 0) {                                            // A (symmetric), b from the 27 sums; the reference's buffer is float
-                int shift = 0;
-                for (int i = 0; i < 6; ++i)
-                    for (int j = i; j < 7; ++j) {
-                        const double value = (double)(float)sums[shift++];
-                        if (j == 6) sb[i] = value; else sA[j * 6 + i] = sA[i * 6 + j] = value;
-                    }
-            }
-            __syncwarp();
-            const int st = chol6_warp(sA, sb, sL, sr);
-            if (lane == 0) {
-                bool good = st == 1;
-                if (st == 2) good = icp_fallback_smem(sA, sb, sr);      // not safely SPD (or NaN): the general path of icp_solve_kernel
-                if (good) icp_compose_pose_smem(sr, Ts);
-                else ok_s = 0;
-            }
-        }
-        __syncthreads();
-    }
-    if (blockIdx.x == 0) {
-        if (tid < 12) T_out[tid] = Ts[tid];
-        if (tid == 0) *ok_out = ok_s;
-    }
-    float acc[27];
-#pragma unroll
-    for (int i = 0; i < 27; ++i) acc[i] = 0.f;
-    if (ok_s) {
-        Aff T;
-        T.r0 = make_float3(Ts[0], Ts[1], Ts[2]); T.r1 = make_float3(Ts[3], Ts[4], Ts[5]); T.r2 = make_float3(Ts[6], Ts[7], Ts[8]);
-        T.t = make_float3(Ts[9], Ts[10], Ts[11]);
-        const int npix = p.cols * p.rows;
-        for (int i = blockIdx.x * NT + tid; i < npix; i += gridDim.x * NT) {
-            const int y = i / p.cols, x = i - y * p.cols;
-            float row[7];
-            if (icp_row<DEPTH>(p, T, x, y, row)) {
-                int k = 0;
-#pragma unroll
-                for (int a = 0; a < 6; ++a)
-#pragma unroll
-                    for (int j = a; j < 7; ++j) acc[k++] += row[a] * row[j];
-            }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 27; ++i) {
-        float v = acc[i];                                               // float warp stage, see icp_accumulate_kernel
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) smem[warp][i] = (double)v;
-    }
-    __syncthreads();
-    if (tid < 27) {
-        double v = 0.0;
-#pragma unroll
-        for (int w = 0; w < NW; ++w) v += smem[w][tid];
-        p.partials[(size_t)blockIdx.x * 27 + tid] = v;
-    }
 }
 
 __global__ void icp_init_kernel(float *T, int *ok)
@@ -755,54 +467,8 @@ int icp_estimate_impl(const float *const *vcurr, const unsigned short *const *dc
                       int *ok_dev, double *scratch, cudaStream_t s)
 {
     if ((size_t)scratch & 15) return (int)cudaErrorMisalignedAddress;
-    // ---- one persistent launch for the whole loop (DF_ICP_PERSISTENT=0: the launch-per-iteration path below) -------------------
-    // Measured slower than the 38 PDL-chained launches -- the serial
-    // 6 x 6 solve + pose composition and the barrier wait are on the critical path either way, and a
-    // PDL launch boundary costs less than a grid barrier plus a redundant reduction in every CTA.  Kept selectable (DF_ICP_PERSISTENT=1),
-    // tested, not the default.
-    static const int persistent = [] { const char *e = getenv("DF_ICP_PERSISTENT"); return e ? atoi(e) : 0; }();
-    if (persistent && levels <= 4) {
-        int dev = 0, sms = DF_NUM_SMS;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        IcpPersistParams q;
-        memset(&q, 0, sizeof q);
-        q.levels = levels;
-        for (int level = 0; level < levels; ++level) {
-            const int div = 1 << level;                      // setLevelIntr, projective_icp.cpp:17-23
-            IcpLevelView &lv = q.lv[level];
-            if (dcurr) { lv.dcurr = dcurr[level]; lv.dprev = dprev[level]; lv.dpitch = dpitch[level]; }
-            else { lv.vcurr = (const float4 *)vcurr[level]; lv.vprev = (const float4 *)vprev[level]; }
-            lv.ncurr = (const float4 *)ncurr[level]; lv.nprev = (const float4 *)nprev[level];
-            lv.pitch = pitch[level];
-            lv.cols = cols[level]; lv.rows = rows[level]; lv.iters = iters[level];
-            lv.fx = intr.fx / div; lv.fy = intr.fy / div; lv.cx = intr.cx / div; lv.cy = intr.cy / div;
-        }
-        q.dist2_thres = dist_thres * dist_thres;             // ComputeIcpHelper ctor, projective_icp.cpp:11-15
-        q.min_cosine = cosf(angle_thres);
-        q.partials = scratch + 32;
-        q.barrier = reinterpret_cast<unsigned int *>(scratch + 28);
-        q.T_out = T_dev; q.ok_out = ok_dev;
-        const int grid = sms < ICP_MAX_PARTIAL_BLOCKS ? sms : ICP_MAX_PARTIAL_BLOCKS;   // one CTA per SM: all co-resident (cooperative launch)
-        if (cudaMemsetAsync(q.barrier, 0, 8, s) != cudaSuccess) return (int)cudaGetLastError();
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(768); cfg.dynamicSmemBytes = 0; cfg.stream = s;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeCooperative;
-        at[0].val.cooperative = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        const cudaError_t le = dcurr ? cudaLaunchKernelEx(&cfg, icp_persistent_kernel<true, 768>, q)
-                                     : cudaLaunchKernelEx(&cfg, icp_persistent_kernel<false, 768>, q);
-        if (le == cudaSuccess) return 0;
-        (void)cudaGetLastError();                            // e.g. the device cannot co-schedule the grid: fall through to the per-iteration path
-    }
-    static const int chained = [] { const char *e = getenv("DF_ICP_CHAINED"); return e ? atoi(e) : 0; }();
-    double *const part0 = scratch + 32;
-    float *Tbuf[2] = {reinterpret_cast<float *>(part0 + 2 * ICP_MAX_PARTIAL_BLOCKS * 27), reinterpret_cast<float *>(part0 + 2 * ICP_MAX_PARTIAL_BLOCKS * 27) + 16};
-    int *okbuf[2] = {reinterpret_cast<int *>(Tbuf[1] + 16), reinterpret_cast<int *>(Tbuf[1] + 16) + 1};
-    icp_init_kernel<<<1, 32, 0, s>>>(chained ? Tbuf[0] : T_dev, chained ? okbuf[0] : ok_dev);        // affine = Identity, projective_icp.cpp:175
+    icp_init_kernel<<<1, 32, 0, s>>>(T_dev, ok_dev);           // affine = Identity, projective_icp.cpp:175
     DF_LAUNCH_CHECK();
-    int cur = 0, prev_blocks = 0, ppar = 0;
     for (int level = levels - 1; level >= 0; --level) {
         const int div = 1 << level;                          // setLevelIntr, projective_icp.cpp:17-23
         IcpParams p;
@@ -821,35 +487,12 @@ int icp_estimate_impl(const float *const *vcurr, const unsigned short *const *dc
         // (tried and dropped, round 1: running the solve as a last-block tail of the accumulate kernel -- the tail's 190 registers
         //  become the whole kernel's allocation, occupancy falls to one block per SM and the stage got slower; replacing the
         //  substitutions' divisions by reciprocal multiplies made the one-thread tail slower, not faster)
-        for (int it = 0; chained && it < iters[level]; ++it) {
-            p.partials = part0 + (size_t)ppar * ICP_MAX_PARTIAL_BLOCKS * 27;
-            const double *prev = part0 + (size_t)(ppar ^ 1) * ICP_MAX_PARTIAL_BLOCKS * 27;
-            const int npix = p.cols * p.rows;
-            int blocks;
-            if (npix >= ICP_MAX_PARTIAL_BLOCKS * 768) {
-                blocks = ICP_MAX_PARTIAL_BLOCKS;
-                if (p.dcurr) launch_pdl(icp_chain_kernel<true, 768>, dim3(blocks), dim3(768), 0, s, p, prev, prev_blocks, (const float *)Tbuf[cur], (const int *)okbuf[cur], Tbuf[cur ^ 1], okbuf[cur ^ 1]);
-                else launch_pdl(icp_chain_kernel<false, 768>, dim3(blocks), dim3(768), 0, s, p, prev, prev_blocks, (const float *)Tbuf[cur], (const int *)okbuf[cur], Tbuf[cur ^ 1], okbuf[cur ^ 1]);
-            } else {
-                blocks = div_up(npix, 256) < ICP_MAX_PARTIAL_BLOCKS ? div_up(npix, 256) : ICP_MAX_PARTIAL_BLOCKS;
-                if (blocks < 1) blocks = 1;
-                if (p.dcurr) launch_pdl(icp_chain_kernel<true, 256>, dim3(blocks), dim3(256), 0, s, p, prev, prev_blocks, (const float *)Tbuf[cur], (const int *)okbuf[cur], Tbuf[cur ^ 1], okbuf[cur ^ 1]);
-                else launch_pdl(icp_chain_kernel<false, 256>, dim3(blocks), dim3(256), 0, s, p, prev, prev_blocks, (const float *)Tbuf[cur], (const int *)okbuf[cur], Tbuf[cur ^ 1], okbuf[cur ^ 1]);
-            }
-            DF_LAUNCH_CHECK();
-            prev_blocks = blocks; ppar ^= 1; cur ^= 1;
-        }
-        for (int it = 0; !chained && it < iters[level]; ++it) {
+        for (int it = 0; it < iters[level]; ++it) {
             const int blocks = launch_accumulate(p, s);
             if (blocks < 0) return -blocks;
             launch_pdl(icp_solve_kernel, dim3(1), dim3(256), 0, s, (const double *)p.partials, blocks, T_dev, ok_dev, (const float *)T_dev, (const int *)ok_dev);
             DF_LAUNCH_CHECK();
         }
-    }
-    if (chained) {                                           // the last iteration's solve; with no iteration at all the pose stays the identity
-        launch_pdl(icp_solve_kernel, dim3(1), dim3(256), 0, s, (const double *)(part0 + (size_t)(ppar ^ 1) * ICP_MAX_PARTIAL_BLOCKS * 27), prev_blocks, T_dev, ok_dev,
-                   (const float *)Tbuf[cur], (const int *)okbuf[cur]);
-        DF_LAUNCH_CHECK();
     }
     return 0;
 }

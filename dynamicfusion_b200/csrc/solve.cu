@@ -1925,9 +1925,11 @@ int dfb::solve_data_term_ev(float *nodes, int M, const void *node_grid, const fl
     }();
     const int ncta = (want == 16 && cluster16 && M >= 256) ? 16 : 8;
     static const int balanced = [] { const char *e = getenv("DF_SOLVE_BALANCED"); return e ? atoi(e) : 1; }();
-    auto launch_cluster = [&](auto kern, size_t smem, auto... args) -> cudaError_t {
-        // function attributes are per device: set them on every launch (cheap) rather than once per process
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto launch_cluster = [&](auto kern, size_t smem_budget, size_t smem, auto... args) -> cudaError_t {
+        // function attributes are per device: set them on every launch (cheap) rather than once per process.  The limit set is the
+        // kernel's fixed budget, never this launch's size: objects advanced from several host threads (df_kinfu_batch_process_host)
+        // share the attribute, and a smaller size set by one thread between another's set and launch would fail that launch
+        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_budget);
         if (ncta == 16) cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(ncta); cfg.blockDim = dim3(LM4_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;
@@ -1953,7 +1955,7 @@ int dfb::solve_data_term_ev(float *nodes, int M, const void *node_grid, const fl
                 const K6 k6 = ncta == 16 ? (K6)solve_lm_v6_kernel<16> : (K6)solve_lm_v6_kernel<8>;
                 static const int trace = [] { const char *e = getenv("DF_SOLVE_TRACE"); return e ? atoi(e) : 0; }();
                 static const int force_fb = [] { const char *e = getenv("DF_SOLVE_V6_FORCE_FALLBACK"); return e ? atoi(e) : 0; }();
-                const cudaError_t le = launch_cluster(k6, Lc6.total, nodes, M, node_grid, ws, nonlinear_iters, linear_iters, stats_dev, cap6, balanced | (force_fb ? 2 : 0) | (trace ? 4 : 0));
+                const cudaError_t le = launch_cluster(k6, budget6, Lc6.total, nodes, M, node_grid, ws, nonlinear_iters, linear_iters, stats_dev, cap6, balanced | (force_fb ? 2 : 0) | (trace ? 4 : 0));
                 if (le != cudaSuccess) return (int)le;
                 v6 = true;
             }
@@ -1964,7 +1966,7 @@ int dfb::solve_data_term_ev(float *nodes, int M, const void *node_grid, const fl
         using KernelT = void (*)(float *, int, const void *, SolveWs, int, int, double *, int, int, int);
         const KernelT kern = ncta == 16 ? (merged ? (KernelT)solve_lm_v5_kernel<16, true> : (KernelT)solve_lm_v5_kernel<16, false>)
                                         : (merged ? (KernelT)solve_lm_v5_kernel<8, true> : (KernelT)solve_lm_v5_kernel<8, false>);
-        const cudaError_t le = launch_cluster(kern, Lc.total, nodes, M, node_grid, ws, nonlinear_iters, linear_iters, stats_dev, cap, balanced, v6 ? 1 : 0);
+        const cudaError_t le = launch_cluster(kern, budget, Lc.total, nodes, M, node_grid, ws, nonlinear_iters, linear_iters, stats_dev, cap, balanced, v6 ? 1 : 0);
         if (le != cudaSuccess) return (int)le;
     } else {
         solve_lm_kernel<<<1, LM_THREADS, 0, s>>>(nodes, M, ws, nonlinear_iters, linear_iters, stats_dev);

@@ -353,11 +353,10 @@ def test_solve_row_overflow_is_loud_and_leaves_the_field_unchanged():
     assert torch.equal(before, wf.nodes_)
 
 
-@pytest.mark.parametrize("env", [{"DF_ICP_PERSISTENT": "1"}, {"DF_ICP_CHAINED": "1"}, {"DF_SOLVE_LM_IMPL": "5", "DF_SOLVE_MERGED": "0"}, {"DF_SOLVE_LM_IMPL": "5", "DF_SOLVE_BALANCED": "0"},
+@pytest.mark.parametrize("env", [{"DF_SOLVE_LM_IMPL": "5", "DF_SOLVE_MERGED": "0"}, {"DF_SOLVE_LM_IMPL": "5", "DF_SOLVE_BALANCED": "0"},
                                  {"DF_SOLVE_V6_FORCE_FALLBACK": "1"}, {"DF_SOLVE_LM_IMPL": "1"}, {"DF_SOLVE_LM_CTAS": "8"}, {"DF_KNN_WARP_LIST": "1"}])
 def test_alternative_icp_and_solve_kernels_in_subprocess(env):
-    """The A/B variants that are selected once per process: the one-launch persistent ICP (grid barrier per iteration), the chained ICP (one launch per
-    iteration with the previous iteration's solve as every CTA's prologue; the default is the two-kernel accumulate + solve chain), the v5 cluster LM
+    """The variants that are selected once per process: the v5 cluster LM
     (two exchanges per PCG step) with two reductions per step / fixed lanes per row, v5 as the fallback the default v6 kernel hands a frame
     to when its halo tables do not fit, the one-block LM fallback, the 8-CTA cluster and the warp-cooperative candidate lists of the 8-NN.  Each re-runs this file's ICP / solve parity tests under
     the switch in a fresh interpreter."""
