@@ -20,31 +20,67 @@ namespace {
 constexpr int MAX_LEVELS = 4;      // ProjectiveICP::MAX_PYRAMID_LEVELS, projective_icp.hpp:12
 constexpr int NSTAGES = 10;
 
-struct Img { void *ptr = nullptr; size_t pitch = 0; int cols = 0, rows = 0; };
+// internal helpers and stages return 0 or a positive status (a cudaError_t value, or what a df_* launcher returned); each extern "C"
+// entry point turns it into its documented convention once, where it returns
+#define CK(call)                                      \
+    do {                                              \
+        const int s__ = (int)(call);                  \
+        if (s__ != 0) return s__;                     \
+    } while (0)
+
+// device memory owned by whoever holds it: freed on destruction, moved (and so swapped) but never copied
+template <class T> struct DevMem {
+    T *p = nullptr;
+    DevMem() = default;
+    DevMem(DevMem &&o) noexcept : p(o.p) { o.p = nullptr; }
+    DevMem &operator=(DevMem &&o) noexcept { std::swap(p, o.p); return *this; }   // what this held is freed with `o`
+    ~DevMem() { if (p) cudaFree(p); }
+    cudaError_t alloc(size_t bytes) { return cudaMalloc((void **)&p, bytes ? bytes : 16); }
+    operator T *() const { return p; }
+};
+
+// a pitched image; `mem` holds `ptr` for the object's own images and is empty in a view of a caller's buffer
+struct Img {
+    void *ptr = nullptr; size_t pitch = 0; int cols = 0, rows = 0;
+    DevMem<void> mem;
+    Img view() const { return Img{ptr, pitch, cols, rows}; }
+};
+
+// getUsedLevelsNum, projective_icp.cpp:110-115
+int used_levels(const df_kinfu_params &p)
+{
+    int i = MAX_LEVELS - 1;
+    for (; i >= 0 && !p.icp_iter_num[i]; --i) {}
+    return i + 1;
+}
+
+int node_capacity(const df_kinfu_params &p) { return p.max_nodes > 0 ? p.max_nodes : (p.cloud_capacity + 49) / 50; }
 
 struct KinFu {
     df_kinfu_params p;
     int device = 0;                       // the CUDA device the object was created on; every entry point switches to it
     cudaStream_t stream = 0;
-    int levels = 0;                       // icp used levels
+    int levels = 0;                       // used_levels(p)
+    int max_nodes_cap = 0;                // node_capacity(p)
+    float vol_pose[12], Rinv_vol[9];      // p.volume_pose as 12 floats, and the inverse of its rotation
     float trunc_dist = 0.f;
     float voxel_size[3];
-    uint32_t *volume = nullptr;
+    DevMem<uint32_t> volume;
     Img depth_in, dists;
     Img cur_depth[MAX_LEVELS], cur_pts[MAX_LEVELS], cur_nrm[MAX_LEVELS], prev_pts[MAX_LEVELS], prev_nrm[MAX_LEVELS];
     Img prev_depth[MAX_LEVELS];           // DF_KINFU_USE_DEPTH only: the model's depth pyramid (prev_.depth_pyr)
     Img canon, canon_nrm, canon_visible;
-    float *cloud = nullptr, *cloud_nrm = nullptr; int *cloud_count = nullptr;
-    float *nodes = nullptr; int M = 0; void *node_grid = nullptr;
-    float *icp_T = nullptr; int *icp_ok = nullptr; double *icp_scratch = nullptr;
-    void *solve_ws = nullptr; size_t solve_ws_bytes = 0; double *solve_stats = nullptr;
-    double *f2_stats = nullptr;
-    void *extract_ws = nullptr; void *project_ws = nullptr;
-    void *integrate_ws = nullptr;
-    void *extend_ws = nullptr; int *M_dev = nullptr;   // df_extend_field workspace / new node count (DF_KINFU_EXTEND_FIELD)
-    void *fusion_ws = nullptr;             // df_integrate_warped workspace (DF_KINFU_WARPED_INTEGRATE)
-    unsigned char *activity = nullptr; size_t activity_bytes = 0;   // dfusion.h DF_ACTIVITY_VOXELS: which stretches of the volume hold surface
-    void *mesh_ws = nullptr; int *mesh_dev = nullptr;   // df_kinfu_mesh: df_mesh_* workspace, {triangles, status}; allocated by the first call
+    DevMem<float> cloud, cloud_nrm; DevMem<int> cloud_count;
+    DevMem<float> nodes; int M = 0; DevMem<void> node_grid;
+    DevMem<float> icp_T; DevMem<int> icp_ok; DevMem<double> icp_scratch;
+    DevMem<void> solve_ws; DevMem<double> solve_stats;
+    DevMem<double> f2_stats;
+    DevMem<void> extract_ws, project_ws;
+    DevMem<void> integrate_ws;
+    DevMem<void> extend_ws; DevMem<int> M_dev;   // df_extend_field workspace / new node count (DF_KINFU_EXTEND_FIELD)
+    DevMem<void> fusion_ws;               // df_integrate_warped workspace (DF_KINFU_WARPED_INTEGRATE)
+    DevMem<unsigned char> activity; size_t activity_bytes = 0;   // dfusion.h DF_ACTIVITY_VOXELS: which stretches of the volume hold surface
+    DevMem<void> mesh_ws; DevMem<int> mesh_dev;   // df_kinfu_mesh: df_mesh_* workspace, {triangles, status}; allocated by the first call
     float *pinned = nullptr;             // 16 floats: T(12) + ok
     std::vector<float> poses;            // 12 floats per pose
     int frame_counter = 0, resets = 0, last_ok = 1, launches = 0;
@@ -52,12 +88,12 @@ struct KinFu {
     std::vector<uint16_t> ov_depth; bool has_ov_depth = false;       // bilateral-filtered depth, dense cols x rows
     float ov_pose[12]; bool has_ov_pose = false;                     // absolute camera pose of the frame
     std::vector<float> ov_nodes; bool has_ov_nodes = false;          // node table after the solve
-    df_f2_params f2; void *f2_ws = nullptr;      // DF_KINFU_F2_SOLVE (SURVEY 8f(2))
+    df_f2_params f2; DevMem<void> f2_ws;  // DF_KINFU_F2_SOLVE (SURVEY 8f(2))
     bool raycast_bricks = true;          // DF_RAYCAST_BRICKS=0: dense march (A/B)
     long long solve_overflows = 0;       // frames whose solve was skipped because a normal-matrix row overflowed (solve.cu ROWCAP); info[11]
     long long last_cloud = -1;
     double host_us[4] = {0, 0, 0, 0}; long long host_frames = 0;   // DF_KINFU_HOSTPROF: launch A, ICP wait, launch B, total
-    unsigned long long *n_upd = nullptr;   // voxels written by the last integrate (filled when DF_KINFU_STAGE_TIMING)
+    DevMem<unsigned long long> n_upd;    // voxels written by the last integrate (filled when DF_KINFU_STAGE_TIMING)
     // Extraction runs on a second stream: nothing later in the frame loop reads the extracted cloud (the reference recomputes it every
     // frame for its host copies, kinfu.cpp:398-399), it only READS the volume, and the volume is not written again before the next
     // frame's integrate -- so it overlaps the ray-cast and the next frame's pre-processing + ICP (mostly launch latency).
@@ -67,26 +103,28 @@ struct KinFu {
                                           // (one 16-SM cluster while the other SMs idle), or as soon as anybody needs the cloud or the volume
     bool extract_pending = false;         // an extraction is in flight on `aux`
     bool overlap_extract = true;          // DF_KINFU_OVERLAP_EXTRACT=0: everything on one stream
-    cudaEvent_t ev[NSTAGES + 1];
-    float stage_ms[NSTAGES];
-    int stage_mark[NSTAGES + 1];
-};
+    cudaEvent_t ev[NSTAGES + 1] = {};
+    float stage_ms[NSTAGES] = {};
+    int stage_mark[NSTAGES + 1] = {};
 
-#define CK(call)                                      \
-    do {                                              \
-        cudaError_t e__ = (call);                     \
-        if (e__ != cudaSuccess) return -(int)e__;     \
-    } while (0)
-#define CKD(call)                                     \
-    do {                                              \
-        int s__ = (call);                             \
-        if (s__ != 0) return -s__;                    \
-    } while (0)
+    // the work queued on both streams finishes before the device memory above is released
+    ~KinFu()
+    {
+        cudaSetDevice(device);
+        cudaStreamSynchronize(stream);
+        if (aux) { cudaStreamSynchronize(aux); cudaStreamDestroy(aux); }
+        for (cudaEvent_t e : {ev_volume_ready, ev_before_lm, ev_extract_done}) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        cudaFreeHost(pinned);
+    }
+};
 
 int alloc_img(Img &im, int rows, int cols, size_t elem)
 {
     im.cols = cols; im.rows = rows; im.pitch = (size_t)cols * elem;     // dense rows (pitch is still carried everywhere)
-    return (int)cudaMalloc(&im.ptr, im.pitch * rows);
+    const cudaError_t e = im.mem.alloc(im.pitch * rows);
+    im.ptr = im.mem;
+    return (int)e;
 }
 
 df_volume vol_of(const KinFu &k)
@@ -146,20 +184,14 @@ __global__ void __launch_bounds__(256) digest_kernel(const uint32_t *__restrict_
     if ((threadIdx.x & 31) == 0) atomicAdd(out, acc);
 }
 
-df_volume vol_of(const KinFu &k);
-
 // the extraction itself (compute_points + compute_normals, tsdf_volume.cpp:313-325) on stream `es`
 int run_extract(KinFu &k, cudaStream_t es)
 {
     const df_kinfu_params &p = k.p;
-    float vol_pose[12], Rinv_vol[9];
-    memcpy(vol_pose, p.volume_pose.R, 36); memcpy(vol_pose + 9, p.volume_pose.t, 12);
-    dfh_mat3_inv(vol_pose, Rinv_vol);
     const df_volume vol = vol_of(k);
-    int st = df_extract_cloud_tracked(vol, p.volume_pose, k.cloud, p.cloud_capacity, k.cloud_count, k.extract_ws, k.activity, es);
-    if (st) return st;
+    CK(df_extract_cloud_tracked(vol, p.volume_pose, k.cloud, p.cloud_capacity, k.cloud_count, k.extract_ws, k.activity, es));
     k.last_cloud = -1;
-    return df_extract_normals(vol, k.cloud, p.cloud_capacity, k.cloud_count, p.volume_pose, Rinv_vol, p.gradient_delta_factor, k.cloud_nrm, es);
+    return df_extract_normals(vol, k.cloud, p.cloud_capacity, k.cloud_count, p.volume_pose, k.Rinv_vol, p.gradient_delta_factor, k.cloud_nrm, es);
 }
 
 // start the deferred extraction on the auxiliary stream once `after` (an event of the main stream) has happened
@@ -229,43 +261,101 @@ void note_solve_overflow(KinFu &k)
     }
 }
 
-static inline double now_us() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool only_df = false)
+// per-frame bookkeeping at the start of df_kinfu_process_* and df_kinfu_dynamicfusion: launch count and stage marks start afresh
+void begin_frame(KinFu &k)
 {
-    const double t_begin = now_us();
-    double t_sync0 = t_begin, t_sync1 = t_begin;
-    const df_kinfu_params &p = k.p;
-    cudaStream_t s = k.stream;
-    const int LEVELS = k.levels;
     k.launches = 0;
     memset(k.stage_mark, 0, sizeof k.stage_mark);
     mark(k, 0);
+}
 
-    if (!only_df) {
-    // ---- pre-processing, kinfu.cpp:226-242 -----------------------------------------------------------------------
-    CKD(df_compute_dists(depth_dev, depth_pitch, p.cols, p.rows, p.intr, (uint16_t *)k.dists.ptr, k.dists.pitch, s));
+static inline double now_us() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+int integrate_rigid(KinFu &k, const float *cam_pose)
+{
+    const df_kinfu_params &p = k.p;
+    const df_volume vol = vol_of(k);
+    float inv[12], vol2cam[12];
+    dfh_aff_inv(cam_pose, inv);
+    dfh_aff_mul(inv, k.vol_pose, vol2cam);                             // camera_pose.inv() * pose_, tsdf_volume.cpp:112
+    k.launches += df_integrate_launch_count(vol);
+    unsigned long long *counter = (p.flags & DF_KINFU_STAGE_TIMING) ? k.n_upd.p : nullptr;
+    if (counter) cudaMemsetAsync(counter, 0, 8, k.stream);
+    if (int w = wait_extract_on_main(k)) return w;                     // write-after-read: the previous frame's extraction reads this volume
+    return df_integrate_tracked(vol, (const uint16_t *)k.dists.ptr, k.dists.pitch, p.cols, p.rows, to_aff(vol2cam), p.intr, counter, k.activity,
+                                k.integrate_ws, k.stream);
+}
+
+int raycast_model(KinFu &k, const float *cam_pose, Img &pts, Img &nrm)
+{
+    const df_kinfu_params &p = k.p;
+    float inv[12], cam2vol[12], Rinv[9];
+    dfh_aff_inv(k.vol_pose, inv);
+    dfh_aff_mul(inv, cam_pose, cam2vol);                               // pose_.inv() * camera_pose, tsdf_volume.cpp:162
+    dfh_mat3_inv(cam2vol, Rinv);
+    ++k.launches;
+    // the loop's own volume is only ever integrated through the activity map, so the march may skip the bricks without negative voxels
+    return df_raycast_points_tracked(vol_of(k), to_aff(cam2vol), Rinv, p.intr, p.cols, p.rows, p.raycast_step_factor, p.gradient_delta_factor,
+                                     (float *)pts.ptr, pts.pitch, (float *)nrm.ptr, nrm.pitch, k.raycast_bricks ? k.activity.p : nullptr, k.stream);
+}
+
+// compute_points + compute_normals, tsdf_volume.cpp:313-325.  needed_now: the caller reads the cloud right after (first frame: node
+// initialisation; field extension): stay on the main stream
+int extract_cloud(KinFu &k, bool needed_now)
+{
+    k.launches += 5;                                                   // count, 2 scans, emit + the normals kernel
+    const bool overlap = k.overlap_extract && !needed_now && !(k.p.flags & DF_KINFU_STAGE_TIMING);
+    if (int w = wait_extract_on_main(k)) return w;                     // an older extraction may still own the cloud buffers
+    if (!overlap) return run_extract(k, k.stream);
+    k.extract_deferred = true;                                         // launched when the next frame's LM/PCG kernel starts, or on demand
+    k.last_cloud = -1;
+    return 0;
+}
+
+int extend_field(KinFu &k)                                             // SURVEY 8f(3) / Report.md step 4, DF_KINFU_EXTEND_FIELD
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    if (!(p.flags & DF_KINFU_EXTEND_FIELD) || k.M <= 0 || k.M >= k.max_nodes_cap) return 0;
+    CK(df_extend_field(k.nodes, k.M, k.max_nodes_cap, k.node_grid, k.cloud, p.cloud_capacity, k.cloud_count, 4,
+                       p.extend_radius > 0 ? p.extend_radius : 0.03f, p.node_step > 0 ? p.node_step : 50, k.M_dev, k.extend_ws, s));
+    k.launches += 3;
+    int Mn = k.M;
+    if (cudaMemcpyAsync(&Mn, k.M_dev, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess) return (int)cudaGetLastError();
+    if (cudaStreamSynchronize(s) != cudaSuccess) return (int)cudaGetLastError();
+    if (Mn == k.M) return 0;
+    k.M = Mn;
+    ++k.launches;
+    return df_build_node_grid(k.nodes, k.M, k.node_grid, s);           // buildKDTree() after the node set changed
+}
+
+// ---- pre-processing, kinfu.cpp:226-242 ---------------------------------------------------------------------------
+int preprocess(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch)
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    CK(df_compute_dists(depth_dev, depth_pitch, p.cols, p.rows, p.intr, (uint16_t *)k.dists.ptr, k.dists.pitch, s));
     if (k.has_ov_depth) {              // lock-step parity hook: the caller's bilateral image instead of this frame's (expf differs by 1 LSB between CUDA and glibc)
         CK(cudaMemcpy2DAsync(k.cur_depth[0].ptr, k.cur_depth[0].pitch, k.ov_depth.data(), (size_t)p.cols * 2, (size_t)p.cols * 2, p.rows, cudaMemcpyHostToDevice, s));
         CK(cudaStreamSynchronize(s));  // the host vector may be replaced right after the call
         k.has_ov_depth = false;
         ++k.launches;
     } else {
-        CKD(df_bilateral(depth_dev, depth_pitch, p.cols, p.rows, (uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch,
-                         p.bilateral_kernel_size, p.bilateral_sigma_spatial, p.bilateral_sigma_depth, s));
+        CK(df_bilateral(depth_dev, depth_pitch, p.cols, p.rows, (uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch,
+                        p.bilateral_kernel_size, p.bilateral_sigma_spatial, p.bilateral_sigma_depth, s));
         k.launches += 2;
     }
     if (p.icp_truncate_depth_dist > 0) {
-        CKD(df_truncate_depth((uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, p.cols, p.rows, p.icp_truncate_depth_dist, s));
+        CK(df_truncate_depth((uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, p.cols, p.rows, p.icp_truncate_depth_dist, s));
         ++k.launches;
     }
-    for (int i = 1; i < LEVELS; ++i) {
-        CKD(df_pyr_down((const uint16_t *)k.cur_depth[i - 1].ptr, k.cur_depth[i - 1].pitch, k.cur_depth[i - 1].cols, k.cur_depth[i - 1].rows,
-                        (uint16_t *)k.cur_depth[i].ptr, k.cur_depth[i].pitch, p.bilateral_sigma_depth, s));
+    for (int i = 1; i < k.levels; ++i) {
+        CK(df_pyr_down((const uint16_t *)k.cur_depth[i - 1].ptr, k.cur_depth[i - 1].pitch, k.cur_depth[i - 1].cols, k.cur_depth[i - 1].rows,
+                       (uint16_t *)k.cur_depth[i].ptr, k.cur_depth[i].pitch, p.bilateral_sigma_depth, s));
         ++k.launches;
     }
     const bool use_depth = (p.flags & DF_KINFU_USE_DEPTH) != 0;
-    for (int i = 0; i < LEVELS; ++i) {
+    for (int i = 0; i < k.levels; ++i) {
         const int div = 1 << i;                                       // Intr::operator()(level), precomp.cpp:10-14
         const df_intr li = {p.intr.fx / div, p.intr.fy / div, p.intr.cx / div, p.intr.cy / div};
         if (use_depth) {
@@ -274,111 +364,69 @@ int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool only_d
             // (kinfu.cpp:284-287), which that build never writes; here it receives what the variable is meant to hold: the vertex map of
             // the level-0 depth (computed before the masking, normals to a scratch map) -- documented divergence, DESIGN 5.
             if (i == 0) {
-                CKD(df_points_normals(li, (const uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, k.cur_depth[0].cols, k.cur_depth[0].rows,
-                                      (float *)k.cur_pts[0].ptr, k.cur_pts[0].pitch, (float *)k.canon_nrm.ptr, k.canon_nrm.pitch, s));
+                CK(df_points_normals(li, (const uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, k.cur_depth[0].cols, k.cur_depth[0].rows,
+                                     (float *)k.cur_pts[0].ptr, k.cur_pts[0].pitch, (float *)k.canon_nrm.ptr, k.canon_nrm.pitch, s));
                 ++k.launches;
             }
-            CKD(df_normals_mask_depth(li, (uint16_t *)k.cur_depth[i].ptr, k.cur_depth[i].pitch, k.cur_depth[i].cols, k.cur_depth[i].rows,
-                                      (float *)k.cur_nrm[i].ptr, k.cur_nrm[i].pitch, s));
+            CK(df_normals_mask_depth(li, (uint16_t *)k.cur_depth[i].ptr, k.cur_depth[i].pitch, k.cur_depth[i].cols, k.cur_depth[i].rows,
+                                     (float *)k.cur_nrm[i].ptr, k.cur_nrm[i].pitch, s));
         } else
-        CKD(df_points_normals(li, (const uint16_t *)k.cur_depth[i].ptr, k.cur_depth[i].pitch, k.cur_depth[i].cols, k.cur_depth[i].rows,
-                              (float *)k.cur_pts[i].ptr, k.cur_pts[i].pitch, (float *)k.cur_nrm[i].ptr, k.cur_nrm[i].pitch, s));
+        CK(df_points_normals(li, (const uint16_t *)k.cur_depth[i].ptr, k.cur_depth[i].pitch, k.cur_depth[i].cols, k.cur_depth[i].rows,
+                             (float *)k.cur_pts[i].ptr, k.cur_pts[i].pitch, (float *)k.cur_nrm[i].ptr, k.cur_nrm[i].pitch, s));
         ++k.launches;
     }
     mark(k, 1);
+    return 0;
+}
+
+// ---- first frame, kinfu.cpp:245-264 --------------------------------------------------------------------------------
+int first_frame(KinFu &k)
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    CK(integrate_rigid(k, &k.poses[k.poses.size() - 12]));
+    CK(extract_cloud(k, true));
+    if (!(p.flags & DF_KINFU_RIGID_ONLY)) {
+        int count = 0;
+        CK(cudaMemcpyAsync(&count, k.cloud_count, sizeof(int), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        k.last_cloud = count;
+        int step = p.node_step > 0 ? p.node_step : 50;
+        int M = (count + step - 1) / step;
+        if (p.max_nodes > 0 && M > p.max_nodes) { step = (count + p.max_nodes - 1) / p.max_nodes; M = (count + step - 1) / step; }
+        k.M = M;
+        if (M > 0) {
+            init_nodes_kernel<<<div_up(M, 256), 256, 0, s>>>((const float4 *)k.cloud.p, step, M, k.nodes);
+            CK(df_build_node_grid(k.nodes, M, k.node_grid, s));        // buildKDTree(), warp_field.cpp:61
+            k.launches += 2;
+        }
     }
-
-    const df_volume vol = vol_of(k);
-    float vol_pose[12];
-    memcpy(vol_pose, p.volume_pose.R, 36); memcpy(vol_pose + 9, p.volume_pose.t, 12);
-    float Rinv_vol[9];
-    dfh_mat3_inv(vol_pose, Rinv_vol);
-
-    auto integrate_with = [&](const Img &dists, const float *cam_pose) -> int {
-        float inv[12], vol2cam[12];
-        dfh_aff_inv(cam_pose, inv);
-        dfh_aff_mul(inv, vol_pose, vol2cam);                           // camera_pose.inv() * pose_, tsdf_volume.cpp:112
-        k.launches += df_integrate_launch_count(vol);
-        unsigned long long *counter = (p.flags & DF_KINFU_STAGE_TIMING) ? k.n_upd : nullptr;
-        if (counter) cudaMemsetAsync(counter, 0, 8, s);
-        if (int w = wait_extract_on_main(k)) return w;                 // write-after-read: the previous frame's extraction reads this volume
-        return df_integrate_tracked(vol, (const uint16_t *)dists.ptr, dists.pitch, p.cols, p.rows, to_aff(vol2cam), p.intr, counter, k.activity, k.integrate_ws, s);
-    };
-    auto raycast_to = [&](const float *cam_pose, Img &pts, Img &nrm) -> int {
-        float inv[12], cam2vol[12], Rinv[9];
-        dfh_aff_inv(vol_pose, inv);
-        dfh_aff_mul(inv, cam_pose, cam2vol);                           // pose_.inv() * camera_pose, tsdf_volume.cpp:162
-        dfh_mat3_inv(cam2vol, Rinv);
-        ++k.launches;
-        // the loop's own volume is only ever integrated through the activity map, so the march may skip the bricks without negative voxels
-        return df_raycast_points_tracked(vol, to_aff(cam2vol), Rinv, p.intr, p.cols, p.rows, p.raycast_step_factor, p.gradient_delta_factor,
-                                         (float *)pts.ptr, pts.pitch, (float *)nrm.ptr, nrm.pitch, k.raycast_bricks ? k.activity : nullptr, s);
-    };
-    auto extract = [&](bool needed_now) -> int {                       // compute_points + compute_normals, tsdf_volume.cpp:313-325
-        // needed_now: the caller reads the cloud right after (first frame: node initialisation; field extension): stay on the main stream
-        k.launches += 5;                                               // count, 2 scans, emit + the normals kernel
-        const bool overlap = k.overlap_extract && !needed_now && !(p.flags & DF_KINFU_STAGE_TIMING);
-        if (int w = wait_extract_on_main(k)) return w;                 // an older extraction may still own the cloud buffers
-        if (!overlap) return run_extract(k, s);
-        k.extract_deferred = true;                                     // launched when the next frame's LM/PCG kernel starts, or on demand
-        k.last_cloud = -1;
-        return 0;
-    };
-
-    auto extend = [&]() -> int {                                       // SURVEY 8f(3) / Report.md step 4, DF_KINFU_EXTEND_FIELD
-        if (!(p.flags & DF_KINFU_EXTEND_FIELD) || k.M <= 0) return 0;
-        const int maxM = p.max_nodes > 0 ? p.max_nodes : (p.cloud_capacity + 49) / 50;
-        if (k.M >= maxM) return 0;
-        int st = df_extend_field(k.nodes, k.M, maxM, k.node_grid, k.cloud, p.cloud_capacity, k.cloud_count, 4,
-                                 p.extend_radius > 0 ? p.extend_radius : 0.03f, p.node_step > 0 ? p.node_step : 50, k.M_dev, k.extend_ws, s);
-        if (st) return st;
-        k.launches += 3;
-        int Mn = k.M;
-        if (cudaMemcpyAsync(&Mn, k.M_dev, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess) return (int)cudaGetLastError();
-        if (cudaStreamSynchronize(s) != cudaSuccess) return (int)cudaGetLastError();
-        if (Mn != k.M) {
-            k.M = Mn;
-            st = df_build_node_grid(k.nodes, k.M, k.node_grid, s);     // buildKDTree() after the node set changed
-            ++k.launches;
-        }
-        return st;
-    };
-
-    // ---- first frame, kinfu.cpp:245-264 ----------------------------------------------------------------------------
-    if (!only_df && k.frame_counter == 0) {
-        CKD(integrate_with(k.dists, &k.poses[k.poses.size() - 12]));
-        CKD(extract(true));
-        if (!(p.flags & DF_KINFU_RIGID_ONLY)) {
-            int count = 0;
-            CK(cudaMemcpyAsync(&count, k.cloud_count, sizeof(int), cudaMemcpyDeviceToHost, s));
-            CK(cudaStreamSynchronize(s));
-            k.last_cloud = count;
-            int step = p.node_step > 0 ? p.node_step : 50;
-            int M = (count + step - 1) / step;
-            if (p.max_nodes > 0 && M > p.max_nodes) { step = (count + p.max_nodes - 1) / p.max_nodes; M = (count + step - 1) / step; }
-            k.M = M;
-            if (M > 0) {
-                init_nodes_kernel<<<div_up(M, 256), 256, 0, s>>>((const float4 *)k.cloud, step, M, k.nodes);
-                CKD(df_build_node_grid(k.nodes, M, k.node_grid, s));       // buildKDTree(), warp_field.cpp:61
-                k.launches += 2;
-            }
-        }
-        for (int i = 0; i < MAX_LEVELS; ++i) {                          // kinfu.cpp:253-261
-            if (p.flags & DF_KINFU_USE_DEPTH) std::swap(k.cur_depth[i], k.prev_depth[i]);
-            else std::swap(k.cur_pts[i], k.prev_pts[i]);
-            std::swap(k.cur_nrm[i], k.prev_nrm[i]);
-        }
-        ++k.frame_counter;
-        return 0;
+    for (int i = 0; i < MAX_LEVELS; ++i) {                              // kinfu.cpp:253-261
+        if (p.flags & DF_KINFU_USE_DEPTH) std::swap(k.cur_depth[i], k.prev_depth[i]);
+        else std::swap(k.cur_pts[i], k.prev_pts[i]);
+        std::swap(k.cur_nrm[i], k.prev_nrm[i]);
     }
+    ++k.frame_counter;
+    return 0;
+}
 
-    // ---- ICP, kinfu.cpp:268-278 (device-resident; one host read of {ok, T}) -----------------------------------------
-    const bool pose_given = !only_df && k.has_ov_pose;               // lock-step parity hook: the caller's pose instead of this frame's ICP
-    if (pose_given) { k.last_ok = 1; CK(cudaStreamSynchronize(s)); note_solve_overflow(k); }
-    if (!only_df && !pose_given) {
+// ---- ICP, kinfu.cpp:268-280 (device-resident; one host read of {ok, T}), or the pose of df_kinfu_set_overrides --------
+// Appends the frame's pose.  ICP failure resets the object (kinfu.cpp:276-277), which leaves frame_counter at 0.
+int track(KinFu &k, double &t_sync0, double &t_sync1)
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    float pose[12];
+    if (k.has_ov_pose) {               // lock-step parity hook: the caller's pose instead of this frame's ICP
+        k.last_ok = 1;
+        CK(cudaStreamSynchronize(s));
+        note_solve_overflow(k);
+        memcpy(pose, k.ov_pose, sizeof pose);
+        k.has_ov_pose = false;
+    } else {
         const float *vc[MAX_LEVELS], *nc[MAX_LEVELS], *vp[MAX_LEVELS], *np[MAX_LEVELS];
         int cols[MAX_LEVELS], rows[MAX_LEVELS]; size_t pitch[MAX_LEVELS];
-        for (int i = 0; i < LEVELS; ++i) {
+        for (int i = 0; i < k.levels; ++i) {
             vc[i] = (const float *)k.cur_pts[i].ptr; nc[i] = (const float *)k.cur_nrm[i].ptr;
             vp[i] = (const float *)k.prev_pts[i].ptr; np[i] = (const float *)k.prev_nrm[i].ptr;
             cols[i] = k.cur_pts[i].cols; rows[i] = k.cur_pts[i].rows; pitch[i] = k.cur_pts[i].pitch;
@@ -386,16 +434,16 @@ int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool only_d
         if (p.flags & DF_KINFU_USE_DEPTH) {                            // estimateTransform(depth pyramids), kinfu.cpp:271
             const unsigned short *dc[MAX_LEVELS], *dp[MAX_LEVELS];
             size_t dpitch[MAX_LEVELS], npitch[MAX_LEVELS];
-            for (int i = 0; i < LEVELS; ++i) {
+            for (int i = 0; i < k.levels; ++i) {
                 dc[i] = (const unsigned short *)k.cur_depth[i].ptr; dp[i] = (const unsigned short *)k.prev_depth[i].ptr;
                 dpitch[i] = k.cur_depth[i].pitch; npitch[i] = k.cur_nrm[i].pitch;
             }
-            CKD(df_icp_estimate_depth(dc, nc, dp, np, cols, rows, dpitch, npitch, LEVELS, p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres,
-                                      k.icp_T, k.icp_ok, k.icp_scratch, s));
+            CK(df_icp_estimate_depth(dc, nc, dp, np, cols, rows, dpitch, npitch, k.levels, p.icp_iter_num, p.intr, p.icp_dist_thres,
+                                     p.icp_angle_thres, k.icp_T, k.icp_ok, k.icp_scratch, s));
         } else
-        CKD(df_icp_estimate(vc, nc, vp, np, cols, rows, pitch, LEVELS, p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres,
-                            k.icp_T, k.icp_ok, k.icp_scratch, s));
-        for (int i = 0; i < LEVELS; ++i) k.launches += 2 * p.icp_iter_num[i];
+        CK(df_icp_estimate(vc, nc, vp, np, cols, rows, pitch, k.levels, p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres,
+                           k.icp_T, k.icp_ok, k.icp_scratch, s));
+        for (int i = 0; i < k.levels; ++i) k.launches += 2 * p.icp_iter_num[i];
         ++k.launches;
         CK(cudaMemcpyAsync(k.pinned, k.icp_T, 12 * sizeof(float), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(k.pinned + 12, k.icp_ok, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -406,132 +454,148 @@ int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool only_d
         memcpy(&ok, k.pinned + 12, sizeof(int));
         k.last_ok = ok;
         note_solve_overflow(k);                                       // the previous frame's solve flag arrived with this sync
-        if (!ok) { CKD(do_reset(k)); return 0; }                      // kinfu.cpp:276-277
+        if (!ok) return do_reset(k);                                  // kinfu.cpp:276-277
+        dfh_aff_mul(&k.poses[k.poses.size() - 12], k.pinned, pose);   // poses_.back() * affine, kinfu.cpp:280
     }
     mark(k, 2);
-    if (pose_given) {
-        k.poses.insert(k.poses.end(), k.ov_pose, k.ov_pose + 12);
-        k.has_ov_pose = false;
-    } else if (!only_df) {
-        float pose[12];
-        dfh_aff_mul(&k.poses[k.poses.size() - 12], k.pinned, pose);   // poses_.back() * affine, kinfu.cpp:280
-        k.poses.insert(k.poses.end(), pose, pose + 12);
-    }
-    const float *cam_pose = &k.poses[k.poses.size() - 12];
-    const int npix = p.cols * p.rows;
+    k.poses.insert(k.poses.end(), pose, pose + 12);
+    return 0;
+}
 
-    if (!(p.flags & DF_KINFU_RIGID_ONLY) && k.M >= 8) {
-        // ---- KinFu::dynamicfusion, kinfu.cpp:344-400 ------------------------------------------------------------------
-        CKD(raycast_to(cam_pose, k.canon_visible, k.canon_nrm));       // tsdf().raycast(camera_pose, ...), :351 (camera frame)
-        float inv_pose[12];
-        dfh_aff_inv(cam_pose, inv_pose);
-        launch_pdl(to_canonical_kernel, dim3(div_up(npix, 256)), dim3(256), 0, s, (const float4 *)k.canon_visible.ptr, make_aff(to_aff(inv_pose)),
-                                                               (float4 *)k.canon.ptr, (float4 *)k.canon_visible.ptr, npix);
-        ++k.launches;
-        mark(k, 3);
-        df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);    // warp_to_live_ stays identity (never set)
-        CKD(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, DF_WARP_IMAGE_COLS(p.cols), nullptr, nullptr, s));   // :385
-        ++k.launches;
-        mark(k, 4);
-        const bool f2_solve = (p.flags & DF_KINFU_F2_SOLVE) != 0;
-        if (f2_solve) {
-            // SURVEY 8f(2): robust 6-DoF data term + regulariser instead of the reference's translation-only data term (opt-in)
-            CKD(df_solve_f2(k.nodes, k.M, k.node_grid, (const float *)k.canon.ptr, (const float *)k.cur_pts[0].ptr, npix, 4, &k.f2, k.f2_stats, k.f2_ws, s));
-            k.launches += 6 + (k.f2.gn_iters + 1) * 4 + k.f2.gn_iters * (3 + 3 * k.f2.lin_iters);
-        } else {
-        CKD(solve_data_term_ev(k.nodes, k.M, k.node_grid, (const float *)k.canon.ptr, (const float *)k.cur_pts[0].ptr, npix, 4,
-                               p.solver_nonlinear_iters, p.solver_linear_iters,
-                               ((p.flags & DF_KINFU_REF_GRAPH_QUIRK) ? DF_SOLVE_REF_GRAPH_QUIRK : 0) | DF_SOLVE_IMAGE_COLS(p.cols), k.solve_stats, k.solve_ws, s,
-                               k.ev_before_lm));   // :387
+// ---- KinFu::dynamicfusion, kinfu.cpp:344-400, at the latest pose ---------------------------------------------------
+// depth: the frame's bilateral-filtered depth, modified in place by project-and-remove; live_pts: its level-0 vertex map.
+// Without a warp field (DF_KINFU_RIGID_ONLY, or fewer than 8 nodes) the frame is integrated rigidly: the plain KinFu (Nerei) loop.
+int dynamicfusion(KinFu &k, const Img &depth, const Img &live_pts)
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    const float *cam_pose = &k.poses[k.poses.size() - 12];
+    if ((p.flags & DF_KINFU_RIGID_ONLY) || k.M < 8) {
+        mark(k, 3); mark(k, 4); mark(k, 5); mark(k, 6); mark(k, 7);
+        CK(integrate_rigid(k, cam_pose));
+        mark(k, 8); mark(k, 9);
+        return 0;
+    }
+    const int npix = p.cols * p.rows;
+    CK(raycast_model(k, cam_pose, k.canon_visible, k.canon_nrm));     // tsdf().raycast(camera_pose, ...), :351 (camera frame)
+    float inv_pose[12];
+    dfh_aff_inv(cam_pose, inv_pose);
+    launch_pdl(to_canonical_kernel, dim3(div_up(npix, 256)), dim3(256), 0, s, (const float4 *)k.canon_visible.ptr, make_aff(to_aff(inv_pose)),
+                                                           (float4 *)k.canon.ptr, (float4 *)k.canon_visible.ptr, npix);
+    ++k.launches;
+    mark(k, 3);
+    df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);    // warp_to_live_ stays identity (never set)
+    CK(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, DF_WARP_IMAGE_COLS(p.cols), nullptr, nullptr, s));   // :385
+    ++k.launches;
+    mark(k, 4);
+    const bool f2_solve = (p.flags & DF_KINFU_F2_SOLVE) != 0;
+    if (f2_solve) {
+        // SURVEY 8f(2): robust 6-DoF data term + regulariser instead of the reference's translation-only data term (opt-in)
+        CK(df_solve_f2(k.nodes, k.M, k.node_grid, (const float *)k.canon.ptr, (const float *)live_pts.ptr, npix, 4, &k.f2, k.f2_stats, k.f2_ws, s));
+        k.launches += 6 + (k.f2.gn_iters + 1) * 4 + k.f2.gn_iters * (3 + 3 * k.f2.lin_iters);
+    } else {
+        CK(solve_data_term_ev(k.nodes, k.M, k.node_grid, (const float *)k.canon.ptr, (const float *)live_pts.ptr, npix, 4,
+                              p.solver_nonlinear_iters, p.solver_linear_iters,
+                              ((p.flags & DF_KINFU_REF_GRAPH_QUIRK) ? DF_SOLVE_REF_GRAPH_QUIRK : 0) | DF_SOLVE_IMAGE_COLS(p.cols), k.solve_stats, k.solve_ws, s,
+                              k.ev_before_lm));   // :387
         k.launches += 9;                                               // prepare, blockscan, scan, tiles, rows (tiles), fill + rows (fallback), lm v6, lm v5 (fallback)
-        CKD(launch_deferred_extract(k, k.ev_before_lm));               // the previous frame's extraction rides on the 132 SMs the solve leaves idle
+        CK(launch_deferred_extract(k, k.ev_before_lm));                // the previous frame's extraction rides on the 132 SMs the solve leaves idle
+    }
+    // row-overflow flag of this solve (stats[5]): lands in pinned memory, looked at after the next stream synchronisation
+    CK(cudaMemcpyAsync(k.pinned + 14, k.solve_stats.p + 5, sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (k.has_ov_nodes) {              // lock-step parity hook: the caller's solved node table (CPU and GPU PCG round differently in the last bits)
+        if (k.ov_nodes.size() == (size_t)k.M * DF_NODE_STRIDE) {
+            CK(cudaMemcpyAsync(k.nodes, k.ov_nodes.data(), k.ov_nodes.size() * 4, cudaMemcpyHostToDevice, s));
+            CK(cudaStreamSynchronize(s));
         }
-        // row-overflow flag of this solve (stats[5]): lands in pinned memory, looked at after the next stream synchronisation
-        CK(cudaMemcpyAsync(k.pinned + 14, k.solve_stats + 5, sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (k.has_ov_nodes) {          // lock-step parity hook: the caller's solved node table (CPU and GPU PCG round differently in the last bits)
-            if (k.ov_nodes.size() == (size_t)k.M * DF_NODE_STRIDE) {
-                CK(cudaMemcpyAsync(k.nodes, k.ov_nodes.data(), k.ov_nodes.size() * 4, cudaMemcpyHostToDevice, s));
-                CK(cudaStreamSynchronize(s));
-            }
-            k.has_ov_nodes = false;
-        }
-        mark(k, 5);
-        if (f2_solve) {
-            CKD(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, 0, nullptr, nullptr, s));
-        } else {
-            // second warp (:389) queries exactly the vertices the solve just built its graph for (CombinedSolver.h:66-84):
-            // re-use those neighbours + weights instead of a third k-NN pass
-            int32_t *knn_idx; float *knn_w;
-            CKD(df_solve_knn_buffers(k.solve_ws, k.M, npix, &knn_idx, &knn_w));
-            CKD(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, DF_WARP_REUSE_KNN, knn_idx, knn_w, s));
-        }
-        ++k.launches;
-        mark(k, 6);
-        if (p.flags & DF_KINFU_WARPED_INTEGRATE) {
-            // SURVEY 8f(1): the update surface_fusion was written towards (tsdf_volume.cpp:240-252) -- every voxel is carried through
-            // the field solved above and fused against the (bilateral-filtered) frame; no pixel is removed, no rigid integrate.
-            mark(k, 7);
-            unsigned long long *counter = (p.flags & DF_KINFU_STAGE_TIMING) ? k.n_upd : nullptr;
-            if (counter) cudaMemsetAsync(counter, 0, 16, s);
-            CKD(df_integrate_warped(vol, (const uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, p.cols, p.rows, p.volume_pose, to_aff(inv_pose),
-                                    p.intr, k.nodes, k.M, k.node_grid, p.fusion_weight_scale, counter, k.activity, k.fusion_ws, s));
-            k.launches += df_integrate_warped_launch_count();
-            mark(k, 8);
-            CKD(extract((p.flags & DF_KINFU_EXTEND_FIELD) != 0));
-            CKD(extend());
-            mark(k, 9);
-        } else {
+        k.has_ov_nodes = false;
+    }
+    mark(k, 5);
+    if (f2_solve) {
+        CK(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, 0, nullptr, nullptr, s));
+    } else {
+        // second warp (:389) queries exactly the vertices the solve just built its graph for (CombinedSolver.h:66-84):
+        // re-use those neighbours + weights instead of a third k-NN pass
+        int32_t *knn_idx; float *knn_w;
+        CK(df_solve_knn_buffers(k.solve_ws, k.M, npix, &knn_idx, &knn_w));
+        CK(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, DF_WARP_REUSE_KNN, knn_idx, knn_w, s));
+    }
+    ++k.launches;
+    mark(k, 6);
+    if (p.flags & DF_KINFU_WARPED_INTEGRATE) {
+        // SURVEY 8f(1): the update surface_fusion was written towards (tsdf_volume.cpp:240-252) -- every voxel is carried through
+        // the field solved above and fused against the (bilateral-filtered) frame; no pixel is removed, no rigid integrate.
+        mark(k, 7);
+        unsigned long long *counter = (p.flags & DF_KINFU_STAGE_TIMING) ? k.n_upd.p : nullptr;
+        if (counter) cudaMemsetAsync(counter, 0, 16, s);
+        CK(df_integrate_warped(vol_of(k), (const uint16_t *)depth.ptr, depth.pitch, p.cols, p.rows, p.volume_pose, to_aff(inv_pose),
+                               p.intr, k.nodes, k.M, k.node_grid, p.fusion_weight_scale, counter, k.activity, k.fusion_ws, s));
+        k.launches += df_integrate_warped_launch_count();
+    } else {
         // surface_fusion (tsdf_volume.cpp:228-255): psdf projects the warped vertices into the (bilateral-filtered) depth,
         // zeroes the pixels they explain, then the ordinary rigid integrate runs on what is left.
-        CKD(df_project_and_remove((uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, p.cols, p.rows, p.intr,
-                                  (float *)k.canon.ptr, k.canon.pitch, p.cols, p.rows, k.project_ws, s));
+        CK(df_project_and_remove((uint16_t *)depth.ptr, depth.pitch, p.cols, p.rows, p.intr, (float *)k.canon.ptr, k.canon.pitch, p.cols, p.rows,
+                                 k.project_ws, s));
         k.launches += 2;
-        CKD(df_compute_dists((const uint16_t *)k.cur_depth[0].ptr, k.cur_depth[0].pitch, p.cols, p.rows, p.intr,
-                             (uint16_t *)k.dists.ptr, k.dists.pitch, s));
+        CK(df_compute_dists((const uint16_t *)depth.ptr, depth.pitch, p.cols, p.rows, p.intr, (uint16_t *)k.dists.ptr, k.dists.pitch, s));
         ++k.launches;
         mark(k, 7);                                                    // stage "integrate" brackets the integrate kernel alone
-        CKD(integrate_with(k.dists, cam_pose));
-        mark(k, 8);
-        CKD(extract((p.flags & DF_KINFU_EXTEND_FIELD) != 0));          // compute_points / compute_normals, :398-399
-        CKD(extend());
-        mark(k, 9);
-        }
-    } else {
-        // plain KinFu (Nerei) loop: integrate the frame rigidly
-        mark(k, 3); mark(k, 4); mark(k, 5); mark(k, 6); mark(k, 7);
-        CKD(integrate_with(k.dists, cam_pose));
-        mark(k, 8); mark(k, 9);
+        CK(integrate_rigid(k, cam_pose));
     }
+    mark(k, 8);
+    CK(extract_cloud(k, (p.flags & DF_KINFU_EXTEND_FIELD) != 0));     // compute_points / compute_normals, :398-399
+    CK(extend_field(k));
+    mark(k, 9);
+    return 0;
+}
 
-    if (only_df) return 1;
-    // ---- ray-cast for the next frame's ICP, kinfu.cpp:297-301 --------------------------------------------------------
-    CKD(raycast_to(cam_pose, k.prev_pts[0], k.prev_nrm[0]));
+// ---- ray-cast for the next frame's ICP, kinfu.cpp:297-301 ------------------------------------------------------------
+int raycast_next(KinFu &k)
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    CK(raycast_model(k, &k.poses[k.poses.size() - 12], k.prev_pts[0], k.prev_nrm[0]));
     if (p.flags & DF_KINFU_USE_DEPTH) {
         // TsdfVolume::raycast(pose, intr, Depth&, Normals&) (tsdf_volume.cu:273-339,441-456) = the same march storing ushort(vertex.z * 1000),
         // then resizeDepthNormals per level (kinfu.cpp:293-295)
-        CKD(df_cloud_to_depth((const float *)k.prev_pts[0].ptr, k.prev_pts[0].pitch, p.cols, p.rows, (uint16_t *)k.prev_depth[0].ptr, k.prev_depth[0].pitch, s));
+        CK(df_cloud_to_depth((const float *)k.prev_pts[0].ptr, k.prev_pts[0].pitch, p.cols, p.rows, (uint16_t *)k.prev_depth[0].ptr, k.prev_depth[0].pitch, s));
         ++k.launches;
-        for (int i = 1; i < LEVELS; ++i) {
-            CKD(df_resize_depth_normals((const uint16_t *)k.prev_depth[i - 1].ptr, k.prev_depth[i - 1].pitch, (const float *)k.prev_nrm[i - 1].ptr,
-                                        k.prev_nrm[i - 1].pitch, k.prev_depth[i - 1].cols, k.prev_depth[i - 1].rows,
-                                        (uint16_t *)k.prev_depth[i].ptr, k.prev_depth[i].pitch, (float *)k.prev_nrm[i].ptr, k.prev_nrm[i].pitch, s));
+        for (int i = 1; i < k.levels; ++i) {
+            CK(df_resize_depth_normals((const uint16_t *)k.prev_depth[i - 1].ptr, k.prev_depth[i - 1].pitch, (const float *)k.prev_nrm[i - 1].ptr,
+                                       k.prev_nrm[i - 1].pitch, k.prev_depth[i - 1].cols, k.prev_depth[i - 1].rows,
+                                       (uint16_t *)k.prev_depth[i].ptr, k.prev_depth[i].pitch, (float *)k.prev_nrm[i].ptr, k.prev_nrm[i].pitch, s));
             ++k.launches;
         }
     } else
-    for (int i = 1; i < LEVELS; ++i) {
-        CKD(df_resize_points_normals((const float *)k.prev_pts[i - 1].ptr, k.prev_pts[i - 1].pitch, (const float *)k.prev_nrm[i - 1].ptr,
-                                     k.prev_nrm[i - 1].pitch, k.prev_pts[i - 1].cols, k.prev_pts[i - 1].rows,
-                                     (float *)k.prev_pts[i].ptr, k.prev_pts[i].pitch, (float *)k.prev_nrm[i].ptr, k.prev_nrm[i].pitch, s));
+    for (int i = 1; i < k.levels; ++i) {
+        CK(df_resize_points_normals((const float *)k.prev_pts[i - 1].ptr, k.prev_pts[i - 1].pitch, (const float *)k.prev_nrm[i - 1].ptr,
+                                    k.prev_nrm[i - 1].pitch, k.prev_pts[i - 1].cols, k.prev_pts[i - 1].rows,
+                                    (float *)k.prev_pts[i].ptr, k.prev_pts[i].pitch, (float *)k.prev_nrm[i].ptr, k.prev_nrm[i].pitch, s));
         ++k.launches;
     }
     mark(k, 10);
+    return 0;
+}
+
+// KinFu::operator()(depth), kinfu.cpp:221-305: the stages in order.  fused = its return value (false: first frame, or tracking lost).
+int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool &fused)
+{
+    const double t_begin = now_us();
+    double t_sync0 = t_begin, t_sync1 = t_begin;
+    fused = false;
+    begin_frame(k);
+    CK(preprocess(k, depth_dev, depth_pitch));
+    if (k.frame_counter == 0) return first_frame(k);
+    CK(track(k, t_sync0, t_sync1));
+    if (k.frame_counter == 0) return 0;                                // tracking lost: the object was reset
+    CK(dynamicfusion(k, k.cur_depth[0], k.cur_pts[0]));
+    CK(raycast_next(k));
     ++k.frame_counter;
-    {
-        const double t_end = now_us();
-        k.host_us[0] += t_sync0 - t_begin; k.host_us[1] += t_sync1 - t_sync0; k.host_us[2] += t_end - t_sync1; k.host_us[3] += t_end - t_begin;
-        ++k.host_frames;
-    }
-    return 1;
+    const double t_end = now_us();
+    k.host_us[0] += t_sync0 - t_begin; k.host_us[1] += t_sync1 - t_sync0; k.host_us[2] += t_end - t_sync1; k.host_us[3] += t_end - t_begin;
+    ++k.host_frames;
+    fused = true;
+    return 0;
 }
 
 }  // namespace
@@ -562,8 +626,6 @@ extern "C" void df_kinfu_default_params(df_kinfu_params *p, int which)
     p->flags = 0;
 }
 
-extern "C" void df_kinfu_destroy(void *kinfu);
-
 extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
 {
     if (pp->volume_dims[0] % 32 != 0) {                               // CV_Assert, kinfu.cpp:97
@@ -590,14 +652,15 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         if (w) k->p.fusion_weight_scale = (float)atof(w);
     }
     const df_kinfu_params &p = k->p;
-    int i = MAX_LEVELS - 1;                                           // getUsedLevelsNum, projective_icp.cpp:110-115
-    for (; i >= 0 && !p.icp_iter_num[i]; --i) {}
-    k->levels = i + 1;
+    k->levels = used_levels(p);
+    k->max_nodes_cap = node_capacity(p);
+    memcpy(k->vol_pose, p.volume_pose.R, 36); memcpy(k->vol_pose + 9, p.volume_pose.t, 12);
+    dfh_mat3_inv(k->vol_pose, k->Rinv_vol);
     float vmax = 0.f;
     for (int d = 0; d < 3; ++d) { k->voxel_size[d] = p.volume_size[d] / p.volume_dims[d]; vmax = vmax > k->voxel_size[d] ? vmax : k->voxel_size[d]; }
     k->trunc_dist = p.tsdf_trunc_dist > 2.1f * vmax ? p.tsdf_trunc_dist : 2.1f * vmax;   // setTruncDist, tsdf_volume.cpp:68-73
     const size_t nvox = (size_t)p.volume_dims[0] * p.volume_dims[1] * p.volume_dims[2];
-    bool ok = cudaMalloc(&k->volume, nvox * 4) == cudaSuccess;
+    bool ok = k->volume.alloc(nvox * 4) == cudaSuccess;
     ok = ok && alloc_img(k->depth_in, p.rows, p.cols, 2) == 0 && alloc_img(k->dists, p.rows, p.cols, 2) == 0;
     int cols = p.cols, rows = p.rows;
     for (int l = 0; l < MAX_LEVELS && ok; ++l) {                      // allocate_buffers, kinfu.cpp:151-194
@@ -608,28 +671,27 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
     }
     ok = ok && alloc_img(k->canon, p.rows, p.cols, 16) == 0 && alloc_img(k->canon_nrm, p.rows, p.cols, 16) == 0 &&
          alloc_img(k->canon_visible, p.rows, p.cols, 16) == 0;
-    ok = ok && cudaMalloc(&k->cloud, (size_t)p.cloud_capacity * 16) == cudaSuccess && cudaMalloc(&k->cloud_nrm, (size_t)p.cloud_capacity * 16) == cudaSuccess;
-    ok = ok && cudaMalloc(&k->cloud_count, 64) == cudaSuccess;
-    const int maxM = p.max_nodes > 0 ? p.max_nodes : (p.cloud_capacity + 49) / 50;
-    ok = ok && cudaMalloc(&k->nodes, (size_t)maxM * DF_NODE_STRIDE * 4) == cudaSuccess && cudaMalloc(&k->node_grid, df_node_grid_bytes(maxM)) == cudaSuccess;
-    ok = ok && cudaMalloc(&k->icp_T, 64) == cudaSuccess && cudaMalloc(&k->icp_ok, 64) == cudaSuccess &&
-         cudaMalloc(&k->icp_scratch, (size_t)DF_ICP_SCRATCH_DOUBLES * 8) == cudaSuccess;
-    k->solve_ws_bytes = df_solve_workspace_bytes(maxM, p.cols * p.rows);
-    ok = ok && cudaMalloc(&k->solve_ws, k->solve_ws_bytes) == cudaSuccess && cudaMalloc(&k->solve_stats, 64) == cudaSuccess;
+    ok = ok && k->cloud.alloc((size_t)p.cloud_capacity * 16) == cudaSuccess && k->cloud_nrm.alloc((size_t)p.cloud_capacity * 16) == cudaSuccess;
+    ok = ok && k->cloud_count.alloc(64) == cudaSuccess;
+    const int maxM = k->max_nodes_cap;
+    ok = ok && k->nodes.alloc((size_t)maxM * DF_NODE_STRIDE * 4) == cudaSuccess && k->node_grid.alloc(df_node_grid_bytes(maxM)) == cudaSuccess;
+    ok = ok && k->icp_T.alloc(64) == cudaSuccess && k->icp_ok.alloc(64) == cudaSuccess &&
+         k->icp_scratch.alloc((size_t)DF_ICP_SCRATCH_DOUBLES * 8) == cudaSuccess;
+    ok = ok && k->solve_ws.alloc(df_solve_workspace_bytes(maxM, p.cols * p.rows)) == cudaSuccess && k->solve_stats.alloc(64) == cudaSuccess;
     k->f2 = df_f2_params{5.0, 0.05, 1e-4, 1e-4, 2, 4, DF_F2_TWIST | DF_F2_TUKEY | DF_F2_HUBER, 30};
     if (p.flags & DF_KINFU_F2_SOLVE)
-        ok = ok && cudaMalloc(&k->f2_ws, df_solve_f2_workspace_bytes(maxM, p.cols * p.rows, 7)) == cudaSuccess && cudaMalloc(&k->f2_stats, 16 * 8) == cudaSuccess;
+        ok = ok && k->f2_ws.alloc(df_solve_f2_workspace_bytes(maxM, p.cols * p.rows, 7)) == cudaSuccess && k->f2_stats.alloc(16 * 8) == cudaSuccess;
     df_volume v = vol_of(*k);
-    ok = ok && cudaMalloc(&k->extract_ws, df_extract_workspace_bytes(v)) == cudaSuccess;
-    ok = ok && cudaMalloc(&k->integrate_ws, df_integrate_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
-    ok = ok && cudaMalloc(&k->extend_ws, df_extend_field_workspace_bytes(p.cloud_capacity)) == cudaSuccess && cudaMalloc((void **)&k->M_dev, 64) == cudaSuccess;
-    ok = ok && cudaMalloc(&k->fusion_ws, df_integrate_warped_workspace_bytes(p.cols, p.rows, maxM)) == cudaSuccess;
+    ok = ok && k->extract_ws.alloc(df_extract_workspace_bytes(v)) == cudaSuccess;
+    ok = ok && k->integrate_ws.alloc(df_integrate_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
+    ok = ok && k->extend_ws.alloc(df_extend_field_workspace_bytes(p.cloud_capacity)) == cudaSuccess && k->M_dev.alloc(64) == cudaSuccess;
+    ok = ok && k->fusion_ws.alloc(df_integrate_warped_workspace_bytes(p.cols, p.rows, maxM)) == cudaSuccess;
     k->activity_bytes = df_volume_activity_bytes(v);
-    ok = ok && cudaMalloc(&k->activity, k->activity_bytes) == cudaSuccess && cudaMemset(k->activity, 0, k->activity_bytes) == cudaSuccess;
-    ok = ok && cudaMalloc(&k->project_ws, df_project_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
+    ok = ok && k->activity.alloc(k->activity_bytes) == cudaSuccess && cudaMemset(k->activity, 0, k->activity_bytes) == cudaSuccess;
+    ok = ok && k->project_ws.alloc(df_project_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
     ok = ok && cudaMemset(k->project_ws, 0, df_project_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
     ok = ok && cudaMemset(k->solve_stats, 0, 64) == cudaSuccess && cudaMemset(k->cloud_count, 0, 64) == cudaSuccess;
-    ok = ok && cudaMallocHost(&k->pinned, 64) == cudaSuccess && (memset(k->pinned, 0, 64), true) && cudaMalloc(&k->n_upd, 64) == cudaSuccess && cudaMemset(k->n_upd, 0, 64) == cudaSuccess;
+    ok = ok && cudaMallocHost(&k->pinned, 64) == cudaSuccess && (memset(k->pinned, 0, 64), true) && k->n_upd.alloc(64) == cudaSuccess && cudaMemset(k->n_upd, 0, 64) == cudaSuccess;
     int prio_lo = 0, prio_hi = 0;
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);              // lo = numerically greatest = lowest priority
     ok = ok && cudaStreamCreateWithPriority(&k->aux, cudaStreamNonBlocking, prio_lo) == cudaSuccess &&
@@ -637,16 +699,19 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
          cudaEventCreateWithFlags(&k->ev_volume_ready, cudaEventDisableTiming) == cudaSuccess &&
          cudaEventCreateWithFlags(&k->ev_extract_done, cudaEventDisableTiming) == cudaSuccess;
     { const char *oe = getenv("DF_KINFU_OVERLAP_EXTRACT"); if (oe && atoi(oe) == 0) k->overlap_extract = false; }
-    for (int e = 0; e <= NSTAGES; ++e) k->ev[e] = nullptr;
     for (int e = 0; e <= NSTAGES && ok; ++e) ok = cudaEventCreate(&k->ev[e]) == cudaSuccess;
     if (!ok) {
         fprintf(stderr, "df_kinfu_create: CUDA allocation failed: %s\n", cudaGetErrorString(cudaGetLastError()));
-        df_kinfu_destroy(k);                                          // frees whatever was allocated (cudaFree(nullptr) is a no-op)
+        delete k;
         return nullptr;
     }
-    memset(k->stage_ms, 0, sizeof k->stage_ms);
-    do_reset(*k);
-    cudaStreamSynchronize(k->stream);
+    int st = do_reset(*k);                                            // an object is only handed out with its volume cleared
+    if (!st) st = (int)cudaStreamSynchronize(k->stream);
+    if (st) {
+        fprintf(stderr, "df_kinfu_create: clearing the volume failed: %s\n", cudaGetErrorString((cudaError_t)st));
+        delete k;
+        return nullptr;
+    }
     return k;
 }
 
@@ -654,29 +719,14 @@ extern "C" void df_kinfu_destroy(void *h)
 {
     KinFu *k = (KinFu *)h;
     if (!k) return;
-    cudaSetDevice(k->device);
     if (getenv("DF_KINFU_HOSTPROF") && k->host_frames)
         fprintf(stderr, "[df_kinfu host profile] frames %lld: launch-A %.1f us, ICP wait %.1f us, launch-B %.1f us, total %.1f us per frame\n", k->host_frames,
                 k->host_us[0] / k->host_frames, k->host_us[1] / k->host_frames, k->host_us[2] / k->host_frames, k->host_us[3] / k->host_frames);
-    cudaStreamSynchronize(k->stream);
-    if (k->aux) { cudaStreamSynchronize(k->aux); cudaStreamDestroy(k->aux); }
-    if (k->ev_volume_ready) cudaEventDestroy(k->ev_volume_ready);
-    if (k->ev_before_lm) cudaEventDestroy(k->ev_before_lm);
-    if (k->ev_extract_done) cudaEventDestroy(k->ev_extract_done);
-    cudaFree(k->volume); cudaFree(k->depth_in.ptr); cudaFree(k->dists.ptr);
-    for (int l = 0; l < MAX_LEVELS; ++l) { cudaFree(k->cur_depth[l].ptr); cudaFree(k->cur_pts[l].ptr); cudaFree(k->cur_nrm[l].ptr); cudaFree(k->prev_pts[l].ptr); cudaFree(k->prev_nrm[l].ptr); cudaFree(k->prev_depth[l].ptr); }
-    cudaFree(k->canon.ptr); cudaFree(k->canon_nrm.ptr); cudaFree(k->canon_visible.ptr);
-    cudaFree(k->cloud); cudaFree(k->cloud_nrm); cudaFree(k->cloud_count); cudaFree(k->nodes); cudaFree(k->node_grid);
-    cudaFree(k->icp_T); cudaFree(k->icp_ok); cudaFree(k->icp_scratch); cudaFree(k->solve_ws); cudaFree(k->solve_stats);
-    cudaFree(k->f2_ws); cudaFree(k->f2_stats);
-    cudaFree(k->extract_ws); cudaFree(k->project_ws); cudaFree(k->activity); cudaFree(k->integrate_ws); cudaFree(k->fusion_ws); cudaFree(k->extend_ws); cudaFree(k->M_dev); cudaFreeHost(k->pinned); cudaFree(k->n_upd);
-    cudaFree(k->mesh_ws); cudaFree(k->mesh_dev);
-    for (int e = 0; e <= NSTAGES; ++e) if (k->ev[e]) cudaEventDestroy(k->ev[e]);
     delete k;
 }
 
 extern "C" int df_kinfu_set_stream(void *h, void *stream) { ((KinFu *)h)->stream = (cudaStream_t)stream; return 0; }
-extern "C" int df_kinfu_reset(void *h) { KinFu *k = (KinFu *)h; int s = do_reset(*k); return s ? -s : 0; }
+extern "C" int df_kinfu_reset(void *h) { return -do_reset(*(KinFu *)h); }
 
 static void finish_timing(KinFu &k)
 {
@@ -713,9 +763,10 @@ extern "C" int df_kinfu_process_device(void *h, const uint16_t *depth_dev, size_
 {
     KinFu *k = (KinFu *)h;
     cudaSetDevice(k->device);
-    const int r = process(*k, depth_dev, pitch);
+    bool fused;
+    const int st = process(*k, depth_dev, pitch, fused);
     finish_timing(*k);
-    return r;
+    return st ? -st : fused;
 }
 
 // KinFu::dynamicfusion(depth, live_frame, current_normals) (kinfu.hpp:87, kinfu.cpp:344-400) as a stand-alone call on
@@ -724,12 +775,11 @@ extern "C" int df_kinfu_dynamicfusion(void *h, uint16_t *depth_dev, size_t depth
 {
     KinFu *k = (KinFu *)h;
     if (k->poses.size() < 12) return 0;
-    const Img saved_depth = k->cur_depth[0], saved_pts = k->cur_pts[0];
-    k->cur_depth[0].ptr = depth_dev; k->cur_depth[0].pitch = depth_pitch;
-    k->cur_pts[0].ptr = (void *)live_points_dev; k->cur_pts[0].pitch = live_pitch;
-    const int r = process(*k, nullptr, 0, true);
-    k->cur_depth[0] = saved_depth; k->cur_pts[0] = saved_pts;
-    return r;
+    begin_frame(*k);
+    mark(*k, 2);                                                      // no tracking: the latest pose is the frame's
+    const Img depth{depth_dev, depth_pitch, k->p.cols, k->p.rows}, live{(void *)live_points_dev, live_pitch, k->p.cols, k->p.rows};
+    const int st = dynamicfusion(*k, depth, live);
+    return st ? -st : 1;
 }
 
 extern "C" int df_kinfu_process_host(void *h, const uint16_t *depth_host, size_t pitch)
@@ -740,12 +790,12 @@ extern "C" int df_kinfu_process_host(void *h, const uint16_t *depth_host, size_t
     cudaError_t e = cudaMemcpy2DAsync(k->depth_in.ptr, k->depth_in.pitch, depth_host, pitch, (size_t)k->p.cols * 2, k->p.rows,
                                       cudaMemcpyHostToDevice, k->stream);
     if (e != cudaSuccess) return -(int)e;
-    const int r = process(*k, (const uint16_t *)k->depth_in.ptr, k->depth_in.pitch);
-    if (r < 0) return r;
+    bool fused;
+    if (int st = process(*k, (const uint16_t *)k->depth_in.ptr, k->depth_in.pitch, fused)) return -st;
     e = cudaStreamSynchronize(k->stream);        // the caller owns the result when the call returns (renderImage / getCameraPose next)
     if (e == cudaSuccess) note_solve_overflow(*k);
     finish_timing(*k);
-    return e == cudaSuccess ? r : -(int)e;
+    return e == cudaSuccess ? fused : -(int)e;
 }
 
 extern "C" int df_kinfu_get_pose(void *h, int time, float *pose12)
@@ -796,18 +846,18 @@ extern "C" int df_kinfu_get_buffer(void *h, int which, void **ptr, size_t *pitch
     Img im;
     switch (which) {
         case 0: im.ptr = k->volume; im.pitch = (size_t)k->p.volume_dims[0] * 4; im.cols = k->p.volume_dims[0]; im.rows = k->p.volume_dims[1] * k->p.volume_dims[2]; break;
-        case 1: im = k->dists; break;
-        case 2: im = k->cur_depth[0]; break;
-        case 3: im = k->cur_pts[0]; break;
-        case 4: im = k->cur_nrm[0]; break;
-        case 5: im = k->prev_pts[0]; break;
-        case 6: im = k->prev_nrm[0]; break;
-        case 7: im = k->canon; break;
-        case 8: im = k->canon_nrm; break;
+        case 1: im = k->dists.view(); break;
+        case 2: im = k->cur_depth[0].view(); break;
+        case 3: im = k->cur_pts[0].view(); break;
+        case 4: im = k->cur_nrm[0].view(); break;
+        case 5: im = k->prev_pts[0].view(); break;
+        case 6: im = k->prev_nrm[0].view(); break;
+        case 7: im = k->canon.view(); break;
+        case 8: im = k->canon_nrm.view(); break;
         case 9: im.ptr = k->cloud; im.pitch = 16; im.cols = 1; im.rows = k->p.cloud_capacity; break;
         case 10: im.ptr = k->cloud_nrm; im.pitch = 16; im.cols = 1; im.rows = k->p.cloud_capacity; break;
         case 11: im.ptr = k->nodes; im.pitch = DF_NODE_STRIDE * 4; im.cols = 1; im.rows = k->M; break;
-        case 12: im = k->canon_visible; break;
+        case 12: im = k->canon_visible.view(); break;
         case 13: im.ptr = k->solve_stats; im.pitch = 64; im.cols = 8; im.rows = 1; break;
         case 15: im.ptr = k->f2_stats; im.pitch = 128; im.cols = 16; im.rows = 1; break;
         case 14: im.ptr = k->activity; im.pitch = k->activity_bytes; im.cols = (int)k->activity_bytes; im.rows = 1; break;
@@ -859,16 +909,15 @@ extern "C" int df_kinfu_state_digest(void *h, unsigned long long *out4_host)
 {
     KinFu *k = (KinFu *)h;
     sync_extract(*k);
-    unsigned long long *d = nullptr;
-    if (cudaMalloc((void **)&d, 32) != cudaSuccess) return (int)cudaGetLastError();
+    DevMem<unsigned long long> d;
+    if (d.alloc(32) != cudaSuccess) return (int)cudaGetLastError();
     cudaMemsetAsync(d, 0, 32, k->stream);
     const size_t nvox = (size_t)k->p.volume_dims[0] * k->p.volume_dims[1] * k->p.volume_dims[2];
     digest_kernel<<<DF_NUM_SMS * 8, 256, 0, k->stream>>>(k->volume, nvox, d);
-    if (k->M > 0) digest_kernel<<<8, 256, 0, k->stream>>>((const uint32_t *)k->nodes, (size_t)k->M * DF_NODE_STRIDE, d + 1);
+    if (k->M > 0) digest_kernel<<<8, 256, 0, k->stream>>>((const uint32_t *)k->nodes.p, (size_t)k->M * DF_NODE_STRIDE, d + 1);
     cudaMemcpyAsync(d + 2, k->cloud_count, sizeof(int), cudaMemcpyDeviceToDevice, k->stream);
     cudaError_t e = cudaMemcpyAsync(out4_host, d, 32, cudaMemcpyDeviceToHost, k->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(k->stream);
-    cudaFree(d);
     if (e != cudaSuccess) return (int)e;
     unsigned long long ph = 0x243f6a8885a308d3ull;                      // camera poses so far, bit pattern by bit pattern
     for (float f : k->poses) { uint32_t u; memcpy(&u, &f, 4); ph = (ph ^ u) * 0x100000001b3ull; }
@@ -887,18 +936,6 @@ extern "C" int df_kinfu_get_stage_ms(void *h, float *ms, int n)
 // ---------------------------------------------------------------------------------------------------------------------------------
 // Snapshots (df_kinfu_save / df_kinfu_load / df_kinfu_snapshot_params; the format is spelled out in dfusion.h)
 namespace {
-
-// the snapshot entry points return 0 or a positive cudaError_t, like the rest of the C ABI
-#define SNAP_CK(call)                                 \
-    do {                                              \
-        cudaError_t e__ = (call);                     \
-        if (e__ != cudaSuccess) return (int)e__;      \
-    } while (0)
-#define SNAP_CKD(call)                                \
-    do {                                              \
-        int s__ = (call);                             \
-        if (s__ != 0) return s__ < 0 ? -s__ : s__;    \
-    } while (0)
 
 constexpr char SNAP_MAGIC[8] = {'D', 'F', 'U', 'S', 'N', 'A', 'P', '\0'};
 constexpr uint32_t SNAP_VERSION = 1;
@@ -938,13 +975,6 @@ struct SnapLayout {
     int levels; size_t activity_bytes, nbricks;
     size_t poses, nodes, activity, pyr, pyr_bytes, cloud, cloud_nrm, classes, payload, total;
 };
-
-int used_levels(const df_kinfu_params &p)
-{
-    int i = MAX_LEVELS - 1;
-    for (; i >= 0 && !p.icp_iter_num[i]; --i) {}
-    return i + 1;
-}
 
 df_volume geometry_of(const df_kinfu_params &p)
 {
@@ -1022,11 +1052,24 @@ int parse_snapshot(const void *buf, size_t bytes, SnapLayout &L)
     return 0;
 }
 
-struct DevBuf {                            // device staging of one save / load, freed on every path
-    void *p = nullptr;
-    ~DevBuf() { cudaFree(p); }
-    cudaError_t alloc(size_t n) { return cudaMalloc(&p, n ? n : 16); }
-};
+// the sections that are object buffers byte for byte, in snapshot order: fn(device pointer, offset in the snapshot, length)
+template <class F> int for_each_buffer_section(KinFu &k, const SnapLayout &L, F &&fn)
+{
+    CK(fn(k.nodes.p, L.nodes, (size_t)L.c.M * DF_NODE_STRIDE * 4));
+    CK(fn(k.activity.p, L.activity, L.activity_bytes));
+    size_t o = L.pyr;
+    for (int l = 0; l < L.levels; ++l) {
+        const Img &first = (k.p.flags & DF_KINFU_USE_DEPTH) ? k.prev_depth[l] : k.prev_pts[l];
+        const Img *ims[2] = {&first, &k.prev_nrm[l]};
+        for (const Img *im : ims) {
+            CK(fn(im->ptr, o, im->pitch * im->rows));
+            o += im->pitch * im->rows;
+        }
+    }
+    CK(fn(k.cloud.p, L.cloud, (size_t)L.c.cloud_count * 16));
+    CK(fn(k.cloud_nrm.p, L.cloud_nrm, (size_t)L.c.cloud_count * 16));
+    return 0;
+}
 
 }  // namespace
 
@@ -1046,52 +1089,39 @@ extern "C" int df_kinfu_save(void *h, void *dst_host, size_t capacity, size_t *b
     cudaSetDevice(k->device);
     cudaStream_t s = k->stream;
     sync_extract(*k);                                                  // the cloud of the last frame is complete
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(cudaStreamSynchronize(s));
     note_solve_overflow(*k);
     SnapLayout L;
     L.p = k->p; L.f2 = k->f2;
     int count = 0;
-    SNAP_CK(cudaMemcpy(&count, k->cloud_count, sizeof count, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&count, k->cloud_count, sizeof count, cudaMemcpyDeviceToHost));
     L.c = SnapCounters{k->frame_counter, k->resets, k->last_ok, k->M, count, (int32_t)(k->poses.size() / 12), k->solve_overflows, 0};
     const df_volume v = vol_of(*k);
-    DevBuf ws, classes, pbytes, payload;
-    SNAP_CK(ws.alloc(df_volume_pack_workspace_bytes(v)));
-    SNAP_CK(classes.alloc(df_volume_brick_count(v)));
-    SNAP_CK(pbytes.alloc(8));
-    SNAP_CKD(df_volume_pack_count(v, ws.p, (unsigned char *)classes.p, (unsigned long long *)pbytes.p, s));
+    DevMem<void> ws; DevMem<unsigned char> classes; DevMem<unsigned long long> pbytes; DevMem<uint32_t> payload;
+    CK(ws.alloc(df_volume_pack_workspace_bytes(v)));
+    CK(classes.alloc(df_volume_brick_count(v)));
+    CK(pbytes.alloc(8));
+    CK(df_volume_pack_count(v, ws, classes, pbytes, s));
     unsigned long long pb = 0;
-    SNAP_CK(cudaMemcpyAsync(&pb, pbytes.p, 8, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(&pb, pbytes, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     L.c.payload_bytes = pb;
     layout_sections(L);
     if (bytes_out) *bytes_out = L.total;
     if (!dst_host) return 0;
     if (capacity < L.total) return (int)cudaErrorInvalidValue;
-    SNAP_CK(payload.alloc(pb));
-    SNAP_CKD(df_volume_pack_emit(v, ws.p, (const unsigned char *)classes.p, (uint32_t *)payload.p, pb, s));
+    CK(payload.alloc(pb));
+    CK(df_volume_pack_emit(v, ws, classes, payload, pb, s));
     unsigned char *b = (unsigned char *)dst_host;
     size_t o = sizeof(SnapHeader);
     memcpy(b + o, &L.p, sizeof L.p); o += sizeof L.p;
     memcpy(b + o, &L.f2, sizeof L.f2); o += sizeof L.f2;
     memcpy(b + o, &L.c, sizeof L.c);
     memcpy(b + L.poses, k->poses.data(), (size_t)L.c.n_poses * 48);
-    SNAP_CK(cudaMemcpyAsync(b + L.nodes, k->nodes, (size_t)k->M * DF_NODE_STRIDE * 4, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaMemcpyAsync(b + L.activity, k->activity, L.activity_bytes, cudaMemcpyDeviceToHost, s));
-    const bool use_depth = (k->p.flags & DF_KINFU_USE_DEPTH) != 0;
-    o = L.pyr;
-    for (int l = 0; l < L.levels; ++l) {
-        const Img &first = use_depth ? k->prev_depth[l] : k->prev_pts[l];
-        const Img *ims[2] = {&first, &k->prev_nrm[l]};
-        for (const Img *im : ims) {
-            SNAP_CK(cudaMemcpyAsync(b + o, im->ptr, im->pitch * im->rows, cudaMemcpyDeviceToHost, s));
-            o += im->pitch * im->rows;
-        }
-    }
-    SNAP_CK(cudaMemcpyAsync(b + L.cloud, k->cloud, (size_t)count * 16, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaMemcpyAsync(b + L.cloud_nrm, k->cloud_nrm, (size_t)count * 16, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaMemcpyAsync(b + L.classes, classes.p, L.nbricks, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaMemcpyAsync(b + L.payload, payload.p, pb, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(for_each_buffer_section(*k, L, [&](void *dev, size_t off, size_t n) { return cudaMemcpyAsync(b + off, dev, n, cudaMemcpyDeviceToHost, s); }));
+    CK(cudaMemcpyAsync(b + L.classes, classes, L.nbricks, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(b + L.payload, payload, pb, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     SnapHeader hd;
     memcpy(hd.magic, SNAP_MAGIC, 8);
     hd.version = SNAP_VERSION; hd.header_bytes = sizeof hd; hd.total_bytes = L.total;
@@ -1107,47 +1137,33 @@ extern "C" int df_kinfu_load(void *h, const void *src_host, size_t bytes)
     SnapLayout L;
     if (int st = parse_snapshot(src_host, bytes, L)) return st;
     if (memcmp(&L.p, &k->p, sizeof L.p) != 0) return reject("parameters differ from the object's");
-    const int maxM = k->p.max_nodes > 0 ? k->p.max_nodes : (k->p.cloud_capacity + 49) / 50;
-    if (L.c.M > maxM) return reject("more nodes than the object can hold");
+    if (L.c.M > k->max_nodes_cap) return reject("more nodes than the object can hold");
     cudaSetDevice(k->device);
     cudaStream_t s = k->stream;
     sync_extract(*k);                                                  // nothing may still read or write the buffers below
     k->extract_pending = false;
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(cudaStreamSynchronize(s));
     note_solve_overflow(*k);
     const unsigned char *b = (const unsigned char *)src_host;
     const df_volume v = vol_of(*k);
-    DevBuf ws, classes, payload, status;
-    SNAP_CK(ws.alloc(df_volume_pack_workspace_bytes(v)));
-    SNAP_CK(classes.alloc(L.nbricks));
-    SNAP_CK(payload.alloc(L.c.payload_bytes));
-    SNAP_CK(status.alloc(sizeof(int)));
-    SNAP_CK(cudaMemcpyAsync(classes.p, b + L.classes, L.nbricks, cudaMemcpyHostToDevice, s));
-    SNAP_CK(cudaMemcpyAsync(payload.p, b + L.payload, L.c.payload_bytes, cudaMemcpyHostToDevice, s));
-    SNAP_CKD(df_volume_unpack(v, (const unsigned char *)classes.p, (const uint32_t *)payload.p, L.c.payload_bytes, ws.p, (int *)status.p, s));
+    DevMem<void> ws; DevMem<unsigned char> classes; DevMem<uint32_t> payload; DevMem<int> status;
+    CK(ws.alloc(df_volume_pack_workspace_bytes(v)));
+    CK(classes.alloc(L.nbricks));
+    CK(payload.alloc(L.c.payload_bytes));
+    CK(status.alloc(sizeof(int)));
+    CK(cudaMemcpyAsync(classes, b + L.classes, L.nbricks, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(payload, b + L.payload, L.c.payload_bytes, cudaMemcpyHostToDevice, s));
+    CK(df_volume_unpack(v, classes, payload, L.c.payload_bytes, ws, status, s));
     int st = 0;
-    SNAP_CK(cudaMemcpyAsync(&st, status.p, sizeof st, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(&st, status, sizeof st, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     if (st == DF_UNPACK_BAD_CLASS) return reject("a brick class byte is not 0, 1 or 2");
     if (st != 0) return reject("payload length differs from what the brick classes imply");
     // the volume is in place; nothing below can fail on the snapshot's contents
-    SNAP_CK(cudaMemcpyAsync(k->nodes, b + L.nodes, (size_t)L.c.M * DF_NODE_STRIDE * 4, cudaMemcpyHostToDevice, s));
-    SNAP_CK(cudaMemcpyAsync(k->activity, b + L.activity, L.activity_bytes, cudaMemcpyHostToDevice, s));
-    const bool use_depth = (k->p.flags & DF_KINFU_USE_DEPTH) != 0;
-    size_t o = L.pyr;
-    for (int l = 0; l < L.levels; ++l) {
-        const Img &first = use_depth ? k->prev_depth[l] : k->prev_pts[l];
-        const Img *ims[2] = {&first, &k->prev_nrm[l]};
-        for (const Img *im : ims) {
-            SNAP_CK(cudaMemcpyAsync(im->ptr, b + o, im->pitch * im->rows, cudaMemcpyHostToDevice, s));
-            o += im->pitch * im->rows;
-        }
-    }
-    SNAP_CK(cudaMemcpyAsync(k->cloud, b + L.cloud, (size_t)L.c.cloud_count * 16, cudaMemcpyHostToDevice, s));
-    SNAP_CK(cudaMemcpyAsync(k->cloud_nrm, b + L.cloud_nrm, (size_t)L.c.cloud_count * 16, cudaMemcpyHostToDevice, s));
-    SNAP_CK(cudaMemcpyAsync(k->cloud_count, &L.c.cloud_count, sizeof(int), cudaMemcpyHostToDevice, s));
-    if (L.c.M > 0) SNAP_CKD(df_build_node_grid(k->nodes, L.c.M, k->node_grid, s));
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(for_each_buffer_section(*k, L, [&](void *dev, size_t off, size_t n) { return cudaMemcpyAsync(dev, b + off, n, cudaMemcpyHostToDevice, s); }));
+    CK(cudaMemcpyAsync(k->cloud_count, &L.c.cloud_count, sizeof(int), cudaMemcpyHostToDevice, s));
+    if (L.c.M > 0) CK(df_build_node_grid(k->nodes, L.c.M, k->node_grid, s));
+    CK(cudaStreamSynchronize(s));
     k->f2 = L.f2;
     k->frame_counter = L.c.frame_counter; k->resets = L.c.resets; k->last_ok = L.c.last_ok; k->M = L.c.M;
     k->solve_overflows = L.c.solve_overflows;
@@ -1165,7 +1181,7 @@ extern "C" int df_kinfu_mesh(void *h, int live, float *verts_host, float *normal
 {
     KinFu *k = (KinFu *)h;
     if (!k || (verts_host && !tris_host)) return (int)cudaErrorInvalidValue;
-    if (live && k->M < 8) {                                            // the loop warps nothing without a field (process(): k.M >= 8)
+    if (live && k->M < 8) {                                            // the loop warps nothing without a field (dynamicfusion(): k.M >= 8)
         fprintf(stderr, "df_kinfu_mesh: no live mesh: the warp field has %d nodes (fewer than 8)\n", k->M);
         return (int)cudaErrorInvalidValue;
     }
@@ -1173,13 +1189,13 @@ extern "C" int df_kinfu_mesh(void *h, int live, float *verts_host, float *normal
     cudaStream_t s = k->stream;
     sync_extract(*k);                                                  // the last frame's cloud is complete
     const df_volume v = vol_of(*k);
-    if (!k->mesh_ws) SNAP_CK(cudaMalloc(&k->mesh_ws, df_mesh_workspace_bytes(v)));
-    if (!k->mesh_dev) SNAP_CK(cudaMalloc((void **)&k->mesh_dev, 64));
-    SNAP_CKD(df_mesh_count(v, k->activity, k->cloud_count, k->mesh_ws, k->mesh_dev, k->mesh_dev + 1, s));
+    if (!k->mesh_ws) CK(k->mesh_ws.alloc(df_mesh_workspace_bytes(v)));
+    if (!k->mesh_dev) CK(k->mesh_dev.alloc(64));
+    CK(df_mesh_count(v, k->activity, k->cloud_count, k->mesh_ws, k->mesh_dev, k->mesh_dev + 1, s));
     int counts[3] = {0, 0, 0};                                         // triangles, status, cloud points
-    SNAP_CK(cudaMemcpyAsync(counts, k->mesh_dev, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaMemcpyAsync(counts + 2, k->cloud_count, sizeof(int), cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(counts, k->mesh_dev, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(counts + 2, k->cloud_count, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     if (counts[1] != 0) {
         fprintf(stderr, "df_kinfu_mesh: the extracted cloud (%d points) does not match the volume: truncated at cloud_capacity (%d), or not "
                         "extracted since the volume last changed\n", counts[2], k->p.cloud_capacity);
@@ -1190,25 +1206,25 @@ extern "C" int df_kinfu_mesh(void *h, int live, float *verts_host, float *normal
     if (n_tris) *n_tris = T;
     if (!verts_host) return 0;
     if (vert_capacity < N || tri_capacity < T) return (int)cudaErrorInvalidValue;
-    DevBuf tris, moved;
-    SNAP_CK(tris.alloc((size_t)T * 12));
-    SNAP_CKD(df_mesh_emit(v, k->activity, k->mesh_ws, (int32_t *)tris.p, T, s));
+    DevMem<int32_t> tris; DevMem<float> moved;
+    CK(tris.alloc((size_t)T * 12));
+    CK(df_mesh_emit(v, k->activity, k->mesh_ws, tris, T, s));
     const float *pts = k->cloud, *nrm = k->cloud_nrm;
     if (live) {                                                        // KinFu::dynamicfusion's warp (kinfu.cpp:385) on copies of the cloud
-        SNAP_CK(moved.alloc((size_t)N * 32));
-        float *mp = (float *)moved.p, *mn = mp + (size_t)N * 4;
-        SNAP_CK(cudaMemcpyAsync(mp, k->cloud, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
-        SNAP_CK(cudaMemcpyAsync(mn, k->cloud_nrm, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
+        CK(moved.alloc((size_t)N * 32));
+        float *mp = moved, *mn = mp + (size_t)N * 4;
+        CK(cudaMemcpyAsync(mp, k->cloud, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(mn, k->cloud_nrm, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
         df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);
-        if (N > 0) SNAP_CKD(df_warp(k->nodes, k->M, k->node_grid, mp, mn, N, 4, ident, 0, nullptr, nullptr, s));
+        if (N > 0) CK(df_warp(k->nodes, k->M, k->node_grid, mp, mn, N, 4, ident, 0, nullptr, nullptr, s));
         pts = mp; nrm = mn;
     }
     std::vector<float> p4((size_t)N * 4), n4(normals_host ? (size_t)N * 4 : 0);
     std::vector<int32_t> t3((size_t)T * 3);
-    SNAP_CK(cudaMemcpyAsync(p4.data(), pts, p4.size() * 4, cudaMemcpyDeviceToHost, s));
-    if (normals_host) SNAP_CK(cudaMemcpyAsync(n4.data(), nrm, n4.size() * 4, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaMemcpyAsync(t3.data(), tris.p, t3.size() * 4, cudaMemcpyDeviceToHost, s));
-    SNAP_CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(p4.data(), pts, p4.size() * 4, cudaMemcpyDeviceToHost, s));
+    if (normals_host) CK(cudaMemcpyAsync(n4.data(), nrm, n4.size() * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(t3.data(), tris, t3.size() * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
     for (size_t i = 0; i < (size_t)N; ++i) {
         memcpy(verts_host + 3 * i, &p4[4 * i], 12);
         if (normals_host) memcpy(normals_host + 3 * i, &n4[4 * i], 12);
