@@ -117,10 +117,6 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
 int solve_data_term_ev(float *nodes, int M, const void *node_grid, const float *canon, const float *live, int N, int stride, int nonlinear_iters,
                        int linear_iters, int flags, double *stats_dev, void *workspace, cudaStream_t stream, cudaEvent_t before_lm);
 
-// Deterministic two-level exclusive scan of n per-block counts (n <= 2^20; extract.cu, also used by snapshot.cu): the exclusive prefix of
-// block i is super[1024 + (i >> 10)] + offsets[i]; *total (device) receives min(sum, capacity).  super: 2048 ints of scratch.
-int scan_block_counts(const int *counts, int n, int *offsets, int *super, int capacity, int *total, cudaStream_t s);
-
 }  // namespace dfb
 
 // first statement of every kernel launched through launch_pdl

@@ -11,6 +11,7 @@
 // Three launches: nearest-node test + per-block counts, a one-block exclusive scan (which also publishes the new node count), and the
 // append (ballot ranks inside the block).  The caller rebuilds the node grid (df_build_node_grid) when the count has changed.
 #include "warp_common.cuh"
+#include "volscan.cuh"
 
 using namespace dfb;
 
@@ -51,28 +52,9 @@ __global__ void __launch_bounds__(256) extend_count_kernel(const float *__restri
 __global__ void __launch_bounds__(1024) extend_scan_kernel(int *block_count, int nblocks, int M, int max_nodes, int step, int *M_out)
 {
     DF_PDL_ENTRY();
-    __shared__ int sm[1024];
-    __shared__ int carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int base = 0; base < nblocks; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int v = i < nblocks ? block_count[i] : 0;
-        sm[threadIdx.x] = v;
-        __syncthreads();
-        for (int o = 1; o < 1024; o <<= 1) {
-            const int t = threadIdx.x >= o ? sm[threadIdx.x - o] : 0;
-            __syncthreads();
-            sm[threadIdx.x] += t;
-            __syncthreads();
-        }
-        if (i < nblocks) block_count[i] = carry + sm[threadIdx.x] - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry += sm[1023];
-        __syncthreads();
-    }
+    const int total = block_scan_in_place(block_count, nblocks);
     if (threadIdx.x == 0) {
-        const long long want = (long long)M + ((long long)carry + step - 1) / step;
+        const long long want = (long long)M + ((long long)total + step - 1) / step;
         *M_out = (int)(want < (long long)max_nodes ? want : (long long)max_nodes);
         if (*M_out < M) *M_out = M;
     }

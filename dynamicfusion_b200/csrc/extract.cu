@@ -6,39 +6,28 @@
 // an exclusive scan over block counts and an emit pass produce the points in ascending (z, y, x) voxel order, +x,+y,+z
 // edge within a voxel -- the same order the CPU oracle uses, so the result is comparable element by element.
 //
-// Work decomposition: the volume is one contiguous array cut into blocks of EX_THREADS quads (1024 voxels when VX = 4), a
-// quad = VX consecutive voxels = one 16-byte load.  A quad whose voxels are all unobserved (W == 0) or free space (F == 1)
-// needs nothing else -- on real scenes that is >90 % of them; only surface quads fetch the +x / +y / +z neighbours (L1/L2
-// hits).  Kernels: see the comment above extract_count_kernel.
-#include "df_common.cuh"
+// Work decomposition: the volume walk of volscan.cuh.  A quad whose voxels are all unobserved (W == 0) or free space (F == 1) needs
+// nothing else -- on real scenes that is >90 % of them; only surface quads fetch the +x / +y / +z neighbours (L1/L2 hits).  Kernels:
+// count (per-block point counts) -> scan_block_counts -> emit (the points of the blocks that have any, at their scanned offsets).  With an
+// activity map the quads of inactive stretches are not loaded at all.
+#include "volscan.cuh"
 
 using namespace dfb;
 
 namespace {
 
-constexpr int EX_THREADS = 256;
-
-struct ExtractParams {
-    const uint32_t *data;
-    int Dx, Dy, Dz;
+struct ExtractParams : VolumeWalk {
     float3 vs;
     Aff pose;
-    size_t nvox;
-    int nblocks;
-    const unsigned char *activity;   // optional (dfusion.h, DF_ACTIVITY_VOXELS): blocks whose stretch of the volume is inactive are skipped
 };
 
-__device__ __forceinline__ float vox_f(uint32_t v) { return half_bits_to_float((unsigned short)(v & 0xffffu)); }
-__device__ __forceinline__ bool sign_change(float F, float Fn) { return (F > 0 && Fn < 0) || (F < 0 && Fn > 0); }
-
-// Calls emit(point) for every zero crossing owned by this thread, in (voxel, axis) order.  tsdf_volume.cu:548-633.
-// the thread's own VX voxels (one 16-byte load when VX = 4); zeros past the end of the volume
+// the thread's quad i: its VX voxels (one 16-byte load when VX = 4), zeros when the quad is skipped
 template <int VX>
 __device__ __forceinline__ void load_quad(const ExtractParams &p, size_t v0, uint32_t (&own)[VX])
 {
 #pragma unroll
     for (int j = 0; j < VX; ++j) own[j] = 0u;
-    if (v0 >= p.nvox) return;
+    if (quad_skipped(p, v0)) return;                                  // an inactive stretch cannot hold surface: not even loaded
     if (VX == 4) {
         const uint4 q = __ldg(reinterpret_cast<const uint4 *>(p.data + v0));
         own[0] = q.x; own[1 % VX] = q.y; own[2 % VX] = q.z; own[3 % VX] = q.w;
@@ -47,6 +36,7 @@ __device__ __forceinline__ void load_quad(const ExtractParams &p, size_t v0, uin
     }
 }
 
+// Calls emit(point) for every zero crossing owned by the quad at v0, in (voxel, axis) order.
 template <int VX, typename Emit>
 __device__ __forceinline__ void thread_crossings(const ExtractParams &p, size_t v0, const uint32_t (&own)[VX], Emit emit)
 {
@@ -54,90 +44,28 @@ __device__ __forceinline__ void thread_crossings(const ExtractParams &p, size_t 
 #pragma unroll
     for (int j = 0; j < VX; ++j) any |= vox_active(own[j]);
     if (!any) return;
-
+    const QuadCoord c = quad_coord(p, v0);
+    if (c.z >= p.Dz - 1) return;                                      // voxel_crossings' bounds, tested before the geometry
     const size_t slice = (size_t)p.Dx * p.Dy;
-    const int z = (int)(v0 / slice);
-    if (z >= p.Dz - 1) return;                               // loop bound z < dims.z - 1, tsdf_volume.cu:553
-    const int rem = (int)(v0 - (size_t)z * slice);
-    const int y = rem / p.Dx;
-    const int x0 = rem - y * p.Dx;
-
 #pragma unroll
     for (int j = 0; j < VX; ++j) {
         if (!vox_active(own[j])) continue;
-        const int x = x0 + j;
         const float F = vox_f(own[j]);
-        const float3 V = make_float3(((float)x + 0.5f) * p.vs.x, ((float)y + 0.5f) * p.vs.y, ((float)z + 0.5f) * p.vs.z);
-        if (x + 1 < p.Dx) {
-            const uint32_t nv = (j + 1 < VX) ? own[(j + 1) % VX] : __ldg(p.data + v0 + VX);
-            if (vox_active(nv)) {
-                const float Fn = vox_f(nv);
-                if (sign_change(F, Fn)) {
-                    const float Vnx = V.x + p.vs.x;
-                    const float d_inv = 1.f / (fabsf(F) + fabsf(Fn));
-                    emit(aff_mul(p.pose, make_float3((V.x * fabsf(Fn) + Vnx * fabsf(F)) * d_inv, V.y, V.z)));
-                }
-            }
-        }
-        if (y + 1 < p.Dy) {
-            const uint32_t nv = __ldg(p.data + v0 + j + p.Dx);
-            if (vox_active(nv)) {
-                const float Fn = vox_f(nv);
-                if (sign_change(F, Fn)) {
-                    const float Vny = V.y + p.vs.y;
-                    const float d_inv = 1.f / (fabsf(F) + fabsf(Fn));
-                    emit(aff_mul(p.pose, make_float3(V.x, (V.y * fabsf(Fn) + Vny * fabsf(F)) * d_inv, V.z)));
-                }
-            }
-        }
-        {
-            const uint32_t nv = __ldg(p.data + v0 + j + slice);
-            if (vox_active(nv)) {
-                const float Fn = vox_f(nv);
-                if (sign_change(F, Fn)) {
-                    const float Vnz = V.z + p.vs.z;
-                    const float d_inv = 1.f / (fabsf(F) + fabsf(Fn));
-                    emit(aff_mul(p.pose, make_float3(V.x, V.y, (V.z * fabsf(Fn) + Vnz * fabsf(F)) * d_inv)));
-                }
-            }
-        }
+        const float3 V = make_float3(((float)(c.x0 + j) + 0.5f) * p.vs.x, ((float)c.y + 0.5f) * p.vs.y, ((float)c.z + 0.5f) * p.vs.z);
+        voxel_crossings(p, own[j], c.x0 + j, c.y, c.z,
+                        [&](int a) {
+                            if (a == 0) return (j + 1 < VX) ? own[(j + 1) % VX] : __ldg(p.data + v0 + VX);
+                            return __ldg(p.data + v0 + j + (a == 1 ? (size_t)p.Dx : slice));
+                        },
+                        [&](int a, float Fn) {                         // the crossing, interpolated between the two voxel centres
+                            const float d_inv = 1.f / (fabsf(F) + fabsf(Fn));
+                            float3 q = V;
+                            if (a == 0) q.x = (V.x * fabsf(Fn) + (V.x + p.vs.x) * fabsf(F)) * d_inv;
+                            else if (a == 1) q.y = (V.y * fabsf(Fn) + (V.y + p.vs.y) * fabsf(F)) * d_inv;
+                            else q.z = (V.z * fabsf(Fn) + (V.z + p.vs.z) * fabsf(F)) * d_inv;
+                            emit(aff_mul(p.pose, q));
+                        });
     }
-}
-
-// Count / emit.  A block = EX_THREADS * EX_QPT quads (4096 voxels when VX = 4), a thread owns quads tid, tid + 256, ...: all of
-// its 16-byte loads are issued before any of them is used, and each load instruction of a warp is one contiguous 512-byte
-// request.  History: one quad per thread meant 131,072 CTAs for 512^3 -- the emit pass, whose CTAs mostly return at once, was
-// limited by block scheduling, not memory; one WARP per block (8 quads per lane, shuffle scans) removed the scheduling cost but
-// serialised the dependent neighbour fetches of the surface quads and was slower still.
-// With an activity map the quads of inactive stretches are not loaded at all.
-constexpr int EX_QPT = 4;
-
-__device__ __forceinline__ int block_exclusive_scan(int v, int *total)
-{
-    __shared__ int warp_sums[EX_THREADS / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int n = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += n;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        int w = lane < EX_THREADS / 32 ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < EX_THREADS / 32; o <<= 1) {
-            const int n = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += n;
-        }
-        if (lane < EX_THREADS / 32) warp_sums[lane] = w;
-    }
-    __syncthreads();
-    const int base = warp ? warp_sums[warp - 1] : 0;
-    if (total) *total = warp_sums[EX_THREADS / 32 - 1];
-    __syncthreads();
-    return base + incl - v;
 }
 
 template <int VX>
@@ -148,101 +76,44 @@ __device__ __forceinline__ int quad_count(const ExtractParams &p, size_t v0, con
     return n;
 }
 
+// all of the thread's 16-byte loads are issued before any of them is used
 template <int VX>
-__device__ __forceinline__ void load_block_quads(const ExtractParams &p, size_t q0, uint32_t (&own)[EX_QPT][VX])
+__device__ __forceinline__ void load_block_quads(const ExtractParams &p, uint32_t (&own)[WALK_QPT][VX])
 {
 #pragma unroll
-    for (int i = 0; i < EX_QPT; ++i) {
-        const size_t v0 = (q0 + (size_t)(i * EX_THREADS) + threadIdx.x) * VX;
-#pragma unroll
-        for (int j = 0; j < VX; ++j) own[i][j] = 0u;
-        if (p.activity && v0 < p.nvox && !p.activity[v0 / DF_ACTIVITY_VOXELS]) continue;    // cannot hold surface: not even loaded
-        load_quad<VX>(p, v0, own[i]);
-    }
+    for (int i = 0; i < WALK_QPT; ++i) load_quad<VX>(p, quad_voxel<VX>(i), own[i]);
 }
 
 template <int VX>
-__global__ void __launch_bounds__(EX_THREADS) extract_count_kernel(const ExtractParams p, int *block_counts)
+__global__ void __launch_bounds__(WALK_THREADS) extract_count_kernel(const ExtractParams p, int *block_counts)
 {
     DF_PDL_ENTRY();
-    const size_t q0 = (size_t)blockIdx.x * EX_THREADS * EX_QPT;
-    uint32_t own[EX_QPT][VX];
-    load_block_quads<VX>(p, q0, own);
+    uint32_t own[WALK_QPT][VX];
+    load_block_quads<VX>(p, own);
     int n = 0;
 #pragma unroll
-    for (int i = 0; i < EX_QPT; ++i) n += quad_count<VX>(p, (q0 + (size_t)(i * EX_THREADS) + threadIdx.x) * VX, own[i]);
+    for (int i = 0; i < WALK_QPT; ++i) n += quad_count<VX>(p, quad_voxel<VX>(i), own[i]);
     const int any = __syncthreads_or(n);
     if (!any) { if (threadIdx.x == 0) block_counts[blockIdx.x] = 0; return; }
     int total;
-    block_exclusive_scan(n, &total);
+    block_exclusive_scan<WALK_THREADS>(n, &total);
     if (threadIdx.x == 0) block_counts[blockIdx.x] = total;
 }
 
-// two-level exclusive scan over the per-block counts: 1024 counts per "super" block (warp-shuffle scan), then one block
-// over the <= 1024 super totals.  (A single-block serial-chunk scan of the 131,072 counts of a 512^3 volume is a long serial chain.)
-__global__ void __launch_bounds__(1024) extract_scan_local_kernel(const int *counts, int *offsets, int n, int *super_tot)
-{
-    DF_PDL_ENTRY();
-    __shared__ int wsum[32];
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    const int i = blockIdx.x * 1024 + t;
-    const int c = i < n ? counts[i] : 0;
-    int incl = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-    if (lane == 31) wsum[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        int w = wsum[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += v; }
-        wsum[lane] = w;
-    }
-    __syncthreads();
-    const int base = warp ? wsum[warp - 1] : 0;
-    if (i < n) offsets[i] = base + incl - c;
-    if (t == 1023) super_tot[blockIdx.x] = wsum[31];
-}
-
-__global__ void __launch_bounds__(1024) extract_scan_super_kernel(const int *super_tot, int nsuper, int *super_off, int capacity, int *count_out)
-{
-    DF_PDL_ENTRY();
-    __shared__ int wsum[32];
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    const int c = t < nsuper ? super_tot[t] : 0;
-    int incl = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-    if (lane == 31) wsum[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        int w = wsum[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += v; }
-        wsum[lane] = w;
-    }
-    __syncthreads();
-    const int base = warp ? wsum[warp - 1] : 0;
-    if (t < nsuper) super_off[t] = base + incl - c;
-    if (t == 1023) *count_out = min(wsum[31], capacity);
-}
-
 template <int VX>
-__global__ void __launch_bounds__(EX_THREADS) extract_emit_kernel(const ExtractParams p, const int *block_counts, const int *offsets,
-                                                                  const int *super_off, float4 *out, int capacity)
+__global__ void __launch_bounds__(WALK_THREADS) extract_emit_kernel(const ExtractParams p, const BlockScan scan, float4 *out, int capacity)
 {
     DF_PDL_ENTRY();
-    if (block_counts[blockIdx.x] == 0) return;
-    const size_t q0 = (size_t)blockIdx.x * EX_THREADS * EX_QPT;
-    uint32_t own[EX_QPT][VX];
-    load_block_quads<VX>(p, q0, own);
-    int run = super_off[blockIdx.x >> 10] + offsets[blockIdx.x];
+    if (scan.counts[blockIdx.x] == 0) return;
+    uint32_t own[WALK_QPT][VX];
+    load_block_quads<VX>(p, own);
+    int run = scan.base(blockIdx.x);
 #pragma unroll
-    for (int i = 0; i < EX_QPT; ++i) {                                // points leave in quad order i * EX_THREADS + tid
-        const size_t v0 = (q0 + (size_t)(i * EX_THREADS) + threadIdx.x) * VX;
+    for (int i = 0; i < WALK_QPT; ++i) {                              // points leave in quad order i * WALK_THREADS + tid
+        const size_t v0 = quad_voxel<VX>(i);
         const int c = quad_count<VX>(p, v0, own[i]);
         int total;
-        int k = run + block_exclusive_scan(c, &total);
+        int k = run + block_exclusive_scan<WALK_THREADS>(c, &total);
         if (c)
             thread_crossings<VX>(p, v0, own[i], [&](const float3 q) {
                 if (k < capacity) out[k] = make_float4(q.x, q.y, q.z, 0.f);
@@ -252,39 +123,13 @@ __global__ void __launch_bounds__(EX_THREADS) extract_emit_kernel(const ExtractP
     }
 }
 
-ExtractParams make_params(const df_volume &vol, const df_aff3f &pose, int vx)
-{
-    ExtractParams p;
-    p.data = vol.data;
-    p.Dx = vol.dims[0]; p.Dy = vol.dims[1]; p.Dz = vol.dims[2];
-    p.vs = make_float3(vol.voxel_size[0], vol.voxel_size[1], vol.voxel_size[2]);
-    p.pose = make_aff(pose);
-    p.nvox = (size_t)vol.dims[0] * vol.dims[1] * vol.dims[2];
-    p.nblocks = (int)((p.nvox + (size_t)EX_THREADS * EX_QPT * vx - 1) / ((size_t)EX_THREADS * EX_QPT * vx));
-    p.activity = nullptr;
-    return p;
-}
-
-int pick_vx(const df_volume &vol) { return (vol.dims[0] % 4 == 0 && ((uintptr_t)vol.data & 15u) == 0) ? 4 : 1; }
-
 }  // namespace
-
-int dfb::scan_block_counts(const int *counts, int n, int *offsets, int *super, int capacity, int *total, cudaStream_t s)
-{
-    const int nsuper = (n + 1023) / 1024;
-    if (nsuper > 1024) return (int)cudaErrorInvalidValue;               // > 2^20 blocks
-    launch_pdl(extract_scan_local_kernel, dim3(nsuper), dim3(1024), 0, s, counts, offsets, n, super);
-    DF_LAUNCH_CHECK();
-    launch_pdl(extract_scan_super_kernel, dim3(1), dim3(1024), 0, s, super, nsuper, super + 1024, capacity, total);
-    DF_LAUNCH_CHECK();
-    return 0;
-}
 
 extern "C" size_t df_extract_workspace_bytes(df_volume vol)
 {
     const size_t nvox = (size_t)vol.dims[0] * vol.dims[1] * vol.dims[2];
-    const size_t nblocks = (nvox + EX_THREADS - 1) / EX_THREADS;          // upper bound (VX = 1)
-    return (2 * nblocks + 2048 + 64) * sizeof(int);
+    const size_t nblocks = (nvox + WALK_THREADS - 1) / WALK_THREADS;      // upper bound (VX = 1)
+    return (block_scan_ints(nblocks) + 64) * sizeof(int);
 }
 
 extern "C" int df_extract_cloud(df_volume vol, df_aff3f pose, float *out_points, int capacity, int *count, void *workspace, void *stream)
@@ -295,19 +140,15 @@ extern "C" int df_extract_cloud(df_volume vol, df_aff3f pose, float *out_points,
 extern "C" int df_extract_cloud_tracked(df_volume vol, df_aff3f pose, float *out_points, int capacity, int *count, void *workspace,
                                         const unsigned char *activity, void *stream)
 {
-    const int vx = pick_vx(vol);
-    ExtractParams p = make_params(vol, pose, vx);
-    p.activity = activity;
-    int *block_counts = (int *)workspace;
-    int *offsets = block_counts + p.nblocks;
+    const ExtractParams p{volume_walk(vol, activity), make_float3(vol.voxel_size[0], vol.voxel_size[1], vol.voxel_size[2]), make_aff(pose)};
+    const BlockScan scan = block_scan_at((int *)workspace, p.nblocks);
     cudaStream_t s = (cudaStream_t)stream;
-    if (vx == 4) launch_pdl(extract_count_kernel<4>, dim3(p.nblocks), dim3(EX_THREADS), 0, s, p, block_counts);
-    else launch_pdl(extract_count_kernel<1>, dim3(p.nblocks), dim3(EX_THREADS), 0, s, p, block_counts);
+    if (p.vx == 4) launch_pdl(extract_count_kernel<4>, dim3(p.nblocks), dim3(WALK_THREADS), 0, s, p, scan.counts);
+    else launch_pdl(extract_count_kernel<1>, dim3(p.nblocks), dim3(WALK_THREADS), 0, s, p, scan.counts);
     DF_LAUNCH_CHECK();
-    int *super_tot = offsets + p.nblocks, *super_off = super_tot + 1024;
-    if (int st = scan_block_counts(block_counts, p.nblocks, offsets, super_tot, capacity, count, s)) return st;   // > 2^20 blocks (volume > 1024^3 voxels)
-    if (vx == 4) launch_pdl(extract_emit_kernel<4>, dim3(p.nblocks), dim3(EX_THREADS), 0, s, p, block_counts, offsets, super_off, (float4 *)out_points, capacity);
-    else launch_pdl(extract_emit_kernel<1>, dim3(p.nblocks), dim3(EX_THREADS), 0, s, p, block_counts, offsets, super_off, (float4 *)out_points, capacity);
+    if (int st = scan_block_counts(scan, p.nblocks, capacity, count, s)) return st;   // > 2^20 blocks (volume > 1024^3 voxels)
+    if (p.vx == 4) launch_pdl(extract_emit_kernel<4>, dim3(p.nblocks), dim3(WALK_THREADS), 0, s, p, scan, (float4 *)out_points, capacity);
+    else launch_pdl(extract_emit_kernel<1>, dim3(p.nblocks), dim3(WALK_THREADS), 0, s, p, scan, (float4 *)out_points, capacity);
     DF_LAUNCH_CHECK();
     return 0;
 }

@@ -1,28 +1,24 @@
 // mesh.cu -- triangle mesh over the extracted cloud (df_mesh_*, dfusion.h), sm_90a.
 //
 // The vertices are the cloud's points (extract.cu), so a triangle is three cloud indices.  The cloud emits its points in ascending
-// (z, y, x) voxel order, +x, +y, +z within a voxel, and the extraction cuts the volume into blocks of MS_THREADS * MS_QPT quads of VX
-// consecutive voxels (the same decomposition is used here).  The cloud index of the point a voxel emits on one axis is then
+// (z, y, x) voxel order, +x, +y, +z within a voxel, over the volume walk of volscan.cuh, and every pass here walks the volume the same way
+// and decides the points by the same crossing rule (crossing_axes).  The cloud index of the point a voxel emits on one axis is then
 //   base[quad of the voxel] + points of the earlier voxels of that quad + points of that voxel on the earlier axes,
-// where base[q] is the index of quad q's first point: its block's offset in the scan of the per-block point counts plus the exclusive scan
-// of the per-quad counts inside the block.  Kernels (all of them over the extraction's blocks):
+// where base[q] is the index of quad q's first point: its block's base in the scan of the per-block point counts plus the exclusive scan
+// of the per-quad counts inside the block.  Kernels:
 //   mesh_count_kernel        per block: cloud points (the recount that validates the cloud) and triangles; one thread per quad of VX cubes
 //                            anchored at the quad's voxels, rows loaded with 16-byte loads when VX = 4;
-//   scan_block_counts x 2    (extract.cu) -> points total, triangle offsets and count;
+//   scan_block_counts x 2    (volscan.cu) -> points total, triangle offsets and count;
 //   mesh_status_kernel       points total against the cloud's count;
 //   mesh_vertex_base_kernel  base[q] for every quad of the blocks that hold points (the table is read only there);
 //   mesh_emit_kernel         the triangles of the blocks that have any, at their scanned offsets.
-// With an activity map, the quads of inactive stretches are skipped by every pass: such a stretch holds no active voxel, so it owns no
-// point and anchors no polygonised cube (its anchor corner would be inactive).
-#include "df_common.cuh"
+// Every pass skips the quads quad_skipped names.
+#include "volscan.cuh"
 #include "../../include/df_mc_table.h"
 
 using namespace dfb;
 
 namespace {
-
-constexpr int MS_THREADS = 256;   // the extraction's EX_THREADS
-constexpr int MS_QPT = 4;         // the extraction's EX_QPT
 
 constexpr signed char kTris[256][DF_MC_ROW] = DF_MC_TRIANGLES_INIT;
 struct TriCounts { unsigned char n[256]; };
@@ -40,22 +36,12 @@ __constant__ TriCounts c_tri_counts = make_tri_counts();
 __constant__ signed char c_tris[256][DF_MC_ROW] = DF_MC_TRIANGLES_INIT;
 __constant__ signed char c_owner[12][4] = DF_MC_EDGE_OWNER_INIT;
 
-struct MeshParams {
-    const uint32_t *data;
-    int Dx, Dy, Dz;
-    size_t nvox;
-    int nblocks, vx;
-    const unsigned char *activity;   // optional (dfusion.h DF_ACTIVITY_VOXELS)
-};
-
-__device__ __forceinline__ float vox_f(uint32_t v) { return half_bits_to_float((unsigned short)(v & 0xffffu)); }
-__device__ __forceinline__ bool sign_change(float F, float Fn) { return (F > 0 && Fn < 0) || (F < 0 && Fn > 0); }
 // a corner of a polygonised cube: active, and F < 0 or F > 0 (not +-0, not NaN)
 __device__ __forceinline__ bool corner_ok(uint32_t v) { const float F = vox_f(v); return vox_active(v) && (F < 0.f || F > 0.f); }
 
 // voxels x0 .. x0 + N - 1 of row (y, z), 0 (inactive) outside the volume; the first VX of them in one 16-byte load when VX = 4
 template <int VX, int N>
-__device__ __forceinline__ void load_row(const MeshParams &p, int x0, int y, int z, uint32_t (&r)[N])
+__device__ __forceinline__ void load_row(const VolumeWalk &p, int x0, int y, int z, uint32_t (&r)[N])
 {
 #pragma unroll
     for (int j = 0; j < N; ++j) r[j] = 0u;
@@ -72,22 +58,10 @@ __device__ __forceinline__ void load_row(const MeshParams &p, int x0, int y, int
         if (x0 + j < p.Dx) r[j] = __ldg(row + x0 + j);
 }
 
-// the cloud points voxel v at (x, y, z) emits, bit a = axis a, exactly as thread_crossings (extract.cu) decides them; n*: its neighbours
-__device__ __forceinline__ int vox_flags(const MeshParams &p, uint32_t v, uint32_t nx, uint32_t ny, uint32_t nz, int x, int y, int z)
-{
-    if (!vox_active(v) || z >= p.Dz - 1) return 0;
-    const float F = vox_f(v);
-    int f = 0;
-    if (x + 1 < p.Dx && vox_active(nx) && sign_change(F, vox_f(nx))) f |= 1;
-    if (y + 1 < p.Dy && vox_active(ny) && sign_change(F, vox_f(ny))) f |= 2;
-    if (vox_active(nz) && sign_change(F, vox_f(nz))) f |= 4;
-    return f;
-}
-
 // case of the cube anchored at (x0 + j, y, z) (dfusion.h: the rule; df_mc_table.h: corner numbering), -1 when it is not polygonised.
 // A, B, C, D: rows (y, z), (y + 1, z), (y, z + 1), (y + 1, z + 1) from x0.
 template <int N>
-__device__ __forceinline__ int cube_case(const MeshParams &p, const uint32_t (&A)[N], const uint32_t (&B)[N], const uint32_t (&C)[N],
+__device__ __forceinline__ int cube_case(const VolumeWalk &p, const uint32_t (&A)[N], const uint32_t (&B)[N], const uint32_t (&C)[N],
                                          const uint32_t (&D)[N], int j, int x0, int y, int z)
 {
     if (x0 + j > p.Dx - 2 || y > p.Dy - 2 || z > p.Dz - 3) return -1;
@@ -101,71 +75,25 @@ __device__ __forceinline__ int cube_case(const MeshParams &p, const uint32_t (&A
     return cs;
 }
 
-struct QuadCoord { int x0, y, z; };
-__device__ __forceinline__ QuadCoord quad_coord(const MeshParams &p, size_t v0)
-{
-    const size_t slice = (size_t)p.Dx * p.Dy;
-    QuadCoord c;
-    c.z = (int)(v0 / slice);
-    const int rem = (int)(v0 - (size_t)c.z * slice);
-    c.y = rem / p.Dx;
-    c.x0 = rem - c.y * p.Dx;
-    return c;
-}
-
-__device__ __forceinline__ bool quad_skipped(const MeshParams &p, size_t v0)
-{
-    return v0 >= p.nvox || (p.activity && !p.activity[v0 / DF_ACTIVITY_VOXELS]);
-}
-
-__device__ __forceinline__ int block_exclusive_scan(int v, int *total)
-{
-    __shared__ int warp_sums[MS_THREADS / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int n = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += n;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        int w = lane < MS_THREADS / 32 ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < MS_THREADS / 32; o <<= 1) {
-            const int n = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += n;
-        }
-        if (lane < MS_THREADS / 32) warp_sums[lane] = w;
-    }
-    __syncthreads();
-    const int base = warp ? warp_sums[warp - 1] : 0;
-    if (total) *total = warp_sums[MS_THREADS / 32 - 1];
-    __syncthreads();
-    return base + incl - v;
-}
-
 // cloud points of the quad at v0 (rows A, B, C from x0, A with one voxel more)
 template <int VX>
-__device__ __forceinline__ int quad_points(const MeshParams &p, const QuadCoord &c, const uint32_t (&A)[VX + 1], const uint32_t (&B)[VX + 1],
+__device__ __forceinline__ int quad_points(const VolumeWalk &p, const QuadCoord &c, const uint32_t (&A)[VX + 1], const uint32_t (&B)[VX + 1],
                                            const uint32_t (&C)[VX + 1])
 {
     int n = 0;
 #pragma unroll
-    for (int j = 0; j < VX; ++j) n += __popc(vox_flags(p, A[j], A[j + 1], B[j], C[j], c.x0 + j, c.y, c.z));
+    for (int j = 0; j < VX; ++j) n += __popc(crossing_axes(p, A[j], A[j + 1], B[j], C[j], c.x0 + j, c.y, c.z));
     return n;
 }
 
 template <int VX>
-__global__ void __launch_bounds__(MS_THREADS) mesh_count_kernel(const MeshParams p, int *point_counts, int *tri_counts)
+__global__ void __launch_bounds__(WALK_THREADS) mesh_count_kernel(const VolumeWalk p, int *point_counts, int *tri_counts)
 {
-    __shared__ int sums[2][MS_THREADS / 32];
-    const size_t q0 = (size_t)blockIdx.x * MS_THREADS * MS_QPT;
+    __shared__ int sums[2][WALK_THREADS / 32];
     int np = 0, nt = 0;
 #pragma unroll
-    for (int i = 0; i < MS_QPT; ++i) {
-        const size_t v0 = (q0 + (size_t)(i * MS_THREADS) + threadIdx.x) * VX;
+    for (int i = 0; i < WALK_QPT; ++i) {
+        const size_t v0 = quad_voxel<VX>(i);
         if (quad_skipped(p, v0)) continue;
         const QuadCoord c = quad_coord(p, v0);
         uint32_t A[VX + 1], B[VX + 1], C[VX + 1], D[VX + 1];
@@ -195,7 +123,7 @@ __global__ void __launch_bounds__(MS_THREADS) mesh_count_kernel(const MeshParams
     if (threadIdx.x == 0) {
         int a = 0, b = 0;
 #pragma unroll
-        for (int w = 0; w < MS_THREADS / 32; ++w) { a += sums[0][w]; b += sums[1][w]; }
+        for (int w = 0; w < WALK_THREADS / 32; ++w) { a += sums[0][w]; b += sums[1][w]; }
         point_counts[blockIdx.x] = a;
         tri_counts[blockIdx.x] = b;
     }
@@ -207,15 +135,13 @@ __global__ void mesh_status_kernel(const int *points_total, const int *cloud_cou
 }
 
 template <int VX>
-__global__ void __launch_bounds__(MS_THREADS) mesh_vertex_base_kernel(const MeshParams p, const int *point_counts, const int *offsets,
-                                                                      const int *super, int *base)
+__global__ void __launch_bounds__(WALK_THREADS) mesh_vertex_base_kernel(const VolumeWalk p, const BlockScan points, int *base)
 {
-    if (point_counts[blockIdx.x] == 0) return;
-    const size_t q0 = (size_t)blockIdx.x * MS_THREADS * MS_QPT;
-    int run = super[1024 + (blockIdx.x >> 10)] + offsets[blockIdx.x];
+    if (points.counts[blockIdx.x] == 0) return;
+    int run = points.base(blockIdx.x);
 #pragma unroll
-    for (int i = 0; i < MS_QPT; ++i) {                              // quads in order i * MS_THREADS + tid, as the cloud's points
-        const size_t v0 = (q0 + (size_t)(i * MS_THREADS) + threadIdx.x) * VX;
+    for (int i = 0; i < WALK_QPT; ++i) {                              // quads in order i * WALK_THREADS + tid, as the cloud's points
+        const size_t v0 = quad_voxel<VX>(i);
         int n = 0;
         if (!quad_skipped(p, v0)) {
             const QuadCoord c = quad_coord(p, v0);
@@ -226,22 +152,21 @@ __global__ void __launch_bounds__(MS_THREADS) mesh_vertex_base_kernel(const Mesh
             n = quad_points<VX>(p, c, A, B, C);
         }
         int total;
-        const int excl = block_exclusive_scan(n, &total);
+        const int excl = block_exclusive_scan<WALK_THREADS>(n, &total);
         if (v0 < p.nvox) base[v0 / VX] = run + excl;
         run += total;
     }
 }
 
 template <int VX>
-__global__ void __launch_bounds__(MS_THREADS) mesh_emit_kernel(const MeshParams p, const int *tri_counts, const int *offsets, const int *super,
-                                                               const int *base, int3 *out, int capacity)
+__global__ void __launch_bounds__(WALK_THREADS) mesh_emit_kernel(const VolumeWalk p, const BlockScan tris, const int *base, int3 *out,
+                                                               int capacity)
 {
-    if (tri_counts[blockIdx.x] == 0) return;
-    const size_t q0 = (size_t)blockIdx.x * MS_THREADS * MS_QPT;
-    int run = super[1024 + (blockIdx.x >> 10)] + offsets[blockIdx.x];
+    if (tris.counts[blockIdx.x] == 0) return;
+    int run = tris.base(blockIdx.x);
 #pragma unroll 1
-    for (int i = 0; i < MS_QPT; ++i) {
-        const size_t v0 = (q0 + (size_t)(i * MS_THREADS) + threadIdx.x) * VX;
+    for (int i = 0; i < WALK_QPT; ++i) {
+        const size_t v0 = quad_voxel<VX>(i);
         QuadCoord c = {0, 0, 0};
         uint32_t A[VX + 2], B[VX + 2], C[VX + 2], D[VX + 2];
         int cs[VX];
@@ -261,7 +186,7 @@ __global__ void __launch_bounds__(MS_THREADS) mesh_emit_kernel(const MeshParams 
             }
         }
         int total;
-        int k = run + block_exclusive_scan(n, &total);
+        int k = run + block_exclusive_scan<WALK_THREADS>(n, &total);
         run += total;
         if (n == 0) continue;
         // the voxels that own this quad's cube edges: rows A, B, C, D (r = dy + 2 dz), voxels x0 .. x0 + VX; their points need the rows
@@ -275,10 +200,10 @@ __global__ void __launch_bounds__(MS_THREADS) mesh_emit_kernel(const MeshParams 
 #pragma unroll
         for (int j = 0; j <= VX; ++j) {
             const int x = c.x0 + j;
-            fl[0][j] = vox_flags(p, A[j], A[j + 1], B[j], C[j], x, c.y, c.z);
-            fl[1][j] = vox_flags(p, B[j], B[j + 1], E[j], D[j], x, c.y + 1, c.z);
-            fl[2][j] = vox_flags(p, C[j], C[j + 1], D[j], F[j], x, c.y, c.z + 1);
-            fl[3][j] = vox_flags(p, D[j], D[j + 1], G[j], H[j], x, c.y + 1, c.z + 1);
+            fl[0][j] = crossing_axes(p, A[j], A[j + 1], B[j], C[j], x, c.y, c.z);
+            fl[1][j] = crossing_axes(p, B[j], B[j + 1], E[j], D[j], x, c.y + 1, c.z);
+            fl[2][j] = crossing_axes(p, C[j], C[j + 1], D[j], F[j], x, c.y, c.z + 1);
+            fl[3][j] = crossing_axes(p, D[j], D[j + 1], G[j], H[j], x, c.y + 1, c.z + 1);
         }
         // cloud index of each owner's first point; voxel x0 + VX is the first of the next quad.  base[] is read only for quads with points.
 #pragma unroll
@@ -312,38 +237,21 @@ __global__ void __launch_bounds__(MS_THREADS) mesh_emit_kernel(const MeshParams 
     }
 }
 
-int pick_vx(const df_volume &vol) { return (vol.dims[0] % 4 == 0 && ((uintptr_t)vol.data & 15u) == 0) ? 4 : 1; }
-
-MeshParams make_params(const df_volume &vol, const unsigned char *activity)
-{
-    MeshParams p;
-    p.data = vol.data;
-    p.Dx = vol.dims[0]; p.Dy = vol.dims[1]; p.Dz = vol.dims[2];
-    p.nvox = (size_t)vol.dims[0] * vol.dims[1] * vol.dims[2];
-    p.vx = pick_vx(vol);
-    const size_t per_block = (size_t)MS_THREADS * MS_QPT * p.vx;
-    p.nblocks = (int)((p.nvox + per_block - 1) / per_block);
-    p.activity = activity;
-    return p;
-}
-
 bool params_ok(const df_volume &vol)
 {
     if (!vol.data || vol.dims[0] <= 0 || vol.dims[1] <= 0 || vol.dims[2] <= 0) return false;
-    return (make_params(vol, nullptr).nblocks + 1023) / 1024 <= 1024;   // scan_block_counts: at most 2^20 blocks
+    return scan_fits(volume_walk(vol, nullptr).nblocks);
 }
 
-struct WsLayout { int *point_counts, *point_offsets, *point_super, *tri_counts, *tri_offsets, *tri_super, *points_total, *base; };
-WsLayout ws_of(void *ws, const MeshParams &p)
+// the scans of the point and triangle counts, the points total (+ 64 ints), then base[] (one int per quad)
+struct WsLayout { BlockScan points, tris; int *points_total, *base; };
+WsLayout ws_of(void *ws, const VolumeWalk &p)
 {
     WsLayout w;
-    w.point_counts = (int *)ws;
-    w.point_offsets = w.point_counts + p.nblocks;
-    w.point_super = w.point_offsets + p.nblocks;
-    w.tri_counts = w.point_super + 2048;
-    w.tri_offsets = w.tri_counts + p.nblocks;
-    w.tri_super = w.tri_offsets + p.nblocks;
-    w.points_total = w.tri_super + 2048;
+    int *q = (int *)ws;
+    w.points = block_scan_at(q, p.nblocks);
+    w.tris = block_scan_at(q += block_scan_ints(p.nblocks), p.nblocks);
+    w.points_total = q + block_scan_ints(p.nblocks);
     w.base = w.points_total + 64;
     return w;
 }
@@ -352,27 +260,27 @@ WsLayout ws_of(void *ws, const MeshParams &p)
 
 extern "C" size_t df_mesh_workspace_bytes(df_volume vol)
 {
-    const MeshParams p = make_params(vol, nullptr);
+    const VolumeWalk p = volume_walk(vol, nullptr);
     const size_t nquads = (p.nvox + p.vx - 1) / p.vx;
-    return (4 * (size_t)p.nblocks + 2 * 2048 + 64 + nquads) * sizeof(int);
+    return (2 * block_scan_ints(p.nblocks) + 64 + nquads) * sizeof(int);
 }
 
 extern "C" int df_mesh_count(df_volume vol, const unsigned char *activity, const int *cloud_count_dev, void *workspace, int *tri_count_dev,
                              int *status_dev, void *stream)
 {
     if (!params_ok(vol) || !cloud_count_dev || !workspace || !tri_count_dev || !status_dev) return (int)cudaErrorInvalidValue;
-    const MeshParams p = make_params(vol, activity);
+    const VolumeWalk p = volume_walk(vol, activity);
     const WsLayout w = ws_of(workspace, p);
     cudaStream_t s = (cudaStream_t)stream;
-    if (p.vx == 4) mesh_count_kernel<4><<<p.nblocks, MS_THREADS, 0, s>>>(p, w.point_counts, w.tri_counts);
-    else mesh_count_kernel<1><<<p.nblocks, MS_THREADS, 0, s>>>(p, w.point_counts, w.tri_counts);
+    if (p.vx == 4) mesh_count_kernel<4><<<p.nblocks, WALK_THREADS, 0, s>>>(p, w.points.counts, w.tris.counts);
+    else mesh_count_kernel<1><<<p.nblocks, WALK_THREADS, 0, s>>>(p, w.points.counts, w.tris.counts);
     DF_LAUNCH_CHECK();
-    if (int st = scan_block_counts(w.point_counts, p.nblocks, w.point_offsets, w.point_super, 0x7fffffff, w.points_total, s)) return st;
-    if (int st = scan_block_counts(w.tri_counts, p.nblocks, w.tri_offsets, w.tri_super, 0x7fffffff, tri_count_dev, s)) return st;
+    if (int st = scan_block_counts(w.points, p.nblocks, 0x7fffffff, w.points_total, s)) return st;
+    if (int st = scan_block_counts(w.tris, p.nblocks, 0x7fffffff, tri_count_dev, s)) return st;
     mesh_status_kernel<<<1, 1, 0, s>>>(w.points_total, cloud_count_dev, status_dev);
     DF_LAUNCH_CHECK();
-    if (p.vx == 4) mesh_vertex_base_kernel<4><<<p.nblocks, MS_THREADS, 0, s>>>(p, w.point_counts, w.point_offsets, w.point_super, w.base);
-    else mesh_vertex_base_kernel<1><<<p.nblocks, MS_THREADS, 0, s>>>(p, w.point_counts, w.point_offsets, w.point_super, w.base);
+    if (p.vx == 4) mesh_vertex_base_kernel<4><<<p.nblocks, WALK_THREADS, 0, s>>>(p, w.points, w.base);
+    else mesh_vertex_base_kernel<1><<<p.nblocks, WALK_THREADS, 0, s>>>(p, w.points, w.base);
     DF_LAUNCH_CHECK();
     return 0;
 }
@@ -380,11 +288,11 @@ extern "C" int df_mesh_count(df_volume vol, const unsigned char *activity, const
 extern "C" int df_mesh_emit(df_volume vol, const unsigned char *activity, const void *workspace, int32_t *tris, int capacity, void *stream)
 {
     if (!params_ok(vol) || !workspace || (!tris && capacity > 0)) return (int)cudaErrorInvalidValue;
-    const MeshParams p = make_params(vol, activity);
+    const VolumeWalk p = volume_walk(vol, activity);
     const WsLayout w = ws_of(const_cast<void *>(workspace), p);
     cudaStream_t s = (cudaStream_t)stream;
-    if (p.vx == 4) mesh_emit_kernel<4><<<p.nblocks, MS_THREADS, 0, s>>>(p, w.tri_counts, w.tri_offsets, w.tri_super, w.base, (int3 *)tris, capacity);
-    else mesh_emit_kernel<1><<<p.nblocks, MS_THREADS, 0, s>>>(p, w.tri_counts, w.tri_offsets, w.tri_super, w.base, (int3 *)tris, capacity);
+    if (p.vx == 4) mesh_emit_kernel<4><<<p.nblocks, WALK_THREADS, 0, s>>>(p, w.tris, w.base, (int3 *)tris, capacity);
+    else mesh_emit_kernel<1><<<p.nblocks, WALK_THREADS, 0, s>>>(p, w.tris, w.base, (int3 *)tris, capacity);
     DF_LAUNCH_CHECK();
     return 0;
 }

@@ -4,12 +4,12 @@
 // is empty (every in-volume voxel 0, what df_clear_volume writes), uniform (every in-volume voxel the same non-zero word: free space) or
 // mixed.  A packed volume is one class byte per brick plus a payload of u32 words in brick order: nothing for an empty brick, its word for
 // a uniform one, its 512 words in (z, y, x) order for a mixed one (slots outside the volume written as 0).  No offsets are stored; both
-// directions derive them with the extraction's deterministic block scan (scan_block_counts, extract.cu).
+// directions derive them with the deterministic block scan of volscan.cuh (scan_block_counts).
 //
 // Work decomposition: one warp per brick, PK_WARPS bricks (consecutive in brick order) per block.  Lane l loads quads l, l + 32, l + 64,
 // l + 96 of the brick (quad j = row j >> 1 = (z, y) = (j >> 4, (j >> 1) & 7), x half j & 1): every 32-byte row of the brick is one sector,
 // and the four 16-byte loads of a lane are independent.
-#include "df_common.cuh"
+#include "volscan.cuh"
 
 using namespace dfb;
 
@@ -43,17 +43,15 @@ bool geom_ok(const df_volume &v)
     if (v.dims[0] <= 0 || v.dims[1] <= 0 || v.dims[2] <= 0 || v.dims[0] % 32 != 0) return false;
     if ((double)v.dims[0] * v.dims[1] * v.dims[2] >= 2147483648.0) return false;
     if (((uintptr_t)v.data & 15u) != 0) return false;
-    return (geom_of(v).nblocks + 1023) / 1024 <= 1024;
+    return scan_fits(geom_of(v).nblocks);
 }
 
-struct WsLayout { int *counts, *offsets, *super, *total, *bad; };
+struct WsLayout { BlockScan scan; int *total, *bad; };
 WsLayout ws_of(void *ws, const PackGeom &g)
 {
     WsLayout w;
-    w.counts = (int *)ws;
-    w.offsets = w.counts + g.nblocks;
-    w.super = w.offsets + g.nblocks;
-    w.total = w.super + 2048;
+    w.scan = block_scan_at((int *)ws, g.nblocks);
+    w.total = (int *)ws + block_scan_ints(g.nblocks);
     w.bad = w.total + 1;
     return w;
 }
@@ -77,9 +75,9 @@ __device__ __forceinline__ long long quad_index(const PackGeom &g, const BrickCo
 }
 
 // exclusive payload offset (words) of the calling warp's brick: block prefix from the scan + the bricks of the earlier warps of the block
-__device__ __forceinline__ int brick_offset(const PackGeom &g, const unsigned char *classes, const int *offsets, const int *super, int warp)
+__device__ __forceinline__ int brick_offset(const PackGeom &g, const unsigned char *classes, const BlockScan &scan, int warp)
 {
-    int off = super[1024 + (blockIdx.x >> 10)] + offsets[blockIdx.x];
+    int off = scan.base(blockIdx.x);
     for (int w = 0; w < warp; ++w) off += class_words(classes[blockIdx.x * PK_WARPS + w]);
     return off;
 }
@@ -124,17 +122,16 @@ __global__ void __launch_bounds__(PK_THREADS) pack_count_kernel(const uint32_t *
 
 // emit: the payload in brick order; only the mixed bricks are read again.  Never writes at or past cap_words.
 __global__ void __launch_bounds__(PK_THREADS) pack_emit_kernel(const uint32_t *__restrict__ vol, const PackGeom g, const unsigned char *classes,
-                                                                const int *block_counts, const int *offsets, const int *super, uint32_t *payload,
-                                                                size_t cap_words)
+                                                                const BlockScan scan, uint32_t *payload, size_t cap_words)
 {
     __shared__ __align__(16) uint32_t stage[PK_WARPS][BRICK_WORDS];
-    if (block_counts[blockIdx.x] == 0) return;
+    if (scan.counts[blockIdx.x] == 0) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int b = blockIdx.x * PK_WARPS + warp;
     if (b >= g.nbricks) return;
     const int cls = classes[b];
     if (cls == 0) return;
-    const size_t off = (size_t)brick_offset(g, classes, offsets, super, warp);
+    const size_t off = (size_t)brick_offset(g, classes, scan, warp);
     const BrickCoord c = brick_coord(g, b);
     if (cls == 1) {
         if (lane == 0 && off < cap_words) payload[off] = vol[((size_t)c.z0 * g.Dy + c.y0) * g.Dx + c.x0];
@@ -184,8 +181,7 @@ __global__ void pack_finish_kernel(const int *total_words, const int *bad, unsig
 
 // unpack, step 2: every voxel of the volume, brick by brick; nothing at all unless the checks passed (*status == 0)
 __global__ void __launch_bounds__(PK_THREADS) unpack_write_kernel(uint32_t *__restrict__ vol, const PackGeom g, const unsigned char *classes,
-                                                                   const int *offsets, const int *super, const uint32_t *__restrict__ payload,
-                                                                   const int *status)
+                                                                   const BlockScan scan, const uint32_t *__restrict__ payload, const int *status)
 {
     __shared__ __align__(16) uint32_t stage[PK_WARPS][BRICK_WORDS];
     if (*status != 0) return;
@@ -194,7 +190,7 @@ __global__ void __launch_bounds__(PK_THREADS) unpack_write_kernel(uint32_t *__re
     if (b >= g.nbricks) return;
     const int cls = classes[b];
     const BrickCoord c = brick_coord(g, b);
-    const size_t off = (size_t)brick_offset(g, classes, offsets, super, warp);
+    const size_t off = (size_t)brick_offset(g, classes, scan, warp);
     if (cls == 2) {
 #pragma unroll
         for (int k = 0; k < BRICK_WORDS / 32; ++k) stage[warp][k * 32 + lane] = __ldg(payload + off + k * 32 + lane);
@@ -217,7 +213,7 @@ extern "C" size_t df_volume_brick_count(df_volume vol) { return (size_t)geom_of(
 
 extern "C" size_t df_volume_pack_workspace_bytes(df_volume vol)
 {
-    return (2 * (size_t)geom_of(vol).nblocks + 2048 + 64) * sizeof(int);
+    return (block_scan_ints(geom_of(vol).nblocks) + 64) * sizeof(int);
 }
 
 extern "C" int df_volume_pack_count(df_volume vol, void *workspace, unsigned char *classes, unsigned long long *payload_bytes, void *stream)
@@ -226,9 +222,9 @@ extern "C" int df_volume_pack_count(df_volume vol, void *workspace, unsigned cha
     const PackGeom g = geom_of(vol);
     const WsLayout w = ws_of(workspace, g);
     cudaStream_t s = (cudaStream_t)stream;
-    pack_count_kernel<<<g.nblocks, PK_THREADS, 0, s>>>(vol.data, g, classes, w.counts);
+    pack_count_kernel<<<g.nblocks, PK_THREADS, 0, s>>>(vol.data, g, classes, w.scan.counts);
     DF_LAUNCH_CHECK();
-    if (int st = scan_block_counts(w.counts, g.nblocks, w.offsets, w.super, 0x7fffffff, w.total, s)) return st;
+    if (int st = scan_block_counts(w.scan, g.nblocks, 0x7fffffff, w.total, s)) return st;
     pack_finish_kernel<<<1, 1, 0, s>>>(w.total, nullptr, 0ull, payload_bytes, nullptr);
     DF_LAUNCH_CHECK();
     return 0;
@@ -239,7 +235,7 @@ extern "C" int df_volume_pack_emit(df_volume vol, const void *workspace, const u
     if (!geom_ok(vol) || !workspace || !classes || (!payload && capacity)) return (int)cudaErrorInvalidValue;
     const PackGeom g = geom_of(vol);
     const WsLayout w = ws_of(const_cast<void *>(workspace), g);
-    pack_emit_kernel<<<g.nblocks, PK_THREADS, 0, (cudaStream_t)stream>>>(vol.data, g, classes, w.counts, w.offsets, w.super, payload, capacity / 4);
+    pack_emit_kernel<<<g.nblocks, PK_THREADS, 0, (cudaStream_t)stream>>>(vol.data, g, classes, w.scan, payload, capacity / 4);
     DF_LAUNCH_CHECK();
     return 0;
 }
@@ -252,12 +248,12 @@ extern "C" int df_volume_unpack(df_volume vol, const unsigned char *classes, con
     const WsLayout w = ws_of(workspace, g);
     cudaStream_t s = (cudaStream_t)stream;
     if (cudaMemsetAsync(w.bad, 0, sizeof(int), s) != cudaSuccess) return (int)cudaGetLastError();
-    unpack_count_kernel<<<div_up(g.nblocks, 256), 256, 0, s>>>(classes, g, w.counts, w.bad);
+    unpack_count_kernel<<<div_up(g.nblocks, 256), 256, 0, s>>>(classes, g, w.scan.counts, w.bad);
     DF_LAUNCH_CHECK();
-    if (int st = scan_block_counts(w.counts, g.nblocks, w.offsets, w.super, 0x7fffffff, w.total, s)) return st;
+    if (int st = scan_block_counts(w.scan, g.nblocks, 0x7fffffff, w.total, s)) return st;
     pack_finish_kernel<<<1, 1, 0, s>>>(w.total, w.bad, (unsigned long long)payload_bytes, nullptr, status);
     DF_LAUNCH_CHECK();
-    unpack_write_kernel<<<g.nblocks, PK_THREADS, 0, s>>>(vol.data, g, classes, w.offsets, w.super, payload, status);
+    unpack_write_kernel<<<g.nblocks, PK_THREADS, 0, s>>>(vol.data, g, classes, w.scan, payload, status);
     DF_LAUNCH_CHECK();
     return 0;
 }

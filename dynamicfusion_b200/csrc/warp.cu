@@ -4,6 +4,7 @@
 // cost, SURVEY.md section 3.4).  The node table (M x 48 B) is GPU-resident; a block stages node positions tile by tile
 // in shared memory and every thread scans them for its own point.
 #include "warp_common.cuh"
+#include "volscan.cuh"
 #include <cstdlib>
 
 using namespace dfb;
@@ -137,26 +138,7 @@ __global__ void __launch_bounds__(256) warp_cursor_count_kernel(const float *__r
 __global__ void __launch_bounds__(1024) warp_cursor_scan_kernel(int *block_count, int nblocks)
 {
     DF_PDL_ENTRY();
-    __shared__ int sm[1024];
-    __shared__ int carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int base = 0; base < nblocks; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int v = i < nblocks ? block_count[i] : 0;
-        sm[threadIdx.x] = v;
-        __syncthreads();
-        for (int o = 1; o < 1024; o <<= 1) {
-            const int t = threadIdx.x >= o ? sm[threadIdx.x - o] : 0;
-            __syncthreads();
-            sm[threadIdx.x] += t;
-            __syncthreads();
-        }
-        if (i < nblocks) block_count[i] = carry + sm[threadIdx.x] - v;        // exclusive
-        __syncthreads();
-        if (threadIdx.x == 1023) carry += sm[1023];
-        __syncthreads();
-    }
+    block_scan_in_place(block_count, nblocks);
 }
 
 __global__ void __launch_bounds__(256) warp_cursor_kernel(const WarpParams p, const int *__restrict__ block_offset, const int *__restrict__ first_nan_normal)

@@ -101,6 +101,7 @@ def test_triangles_equal_the_oracle():
         for use_activity in (False, True):
             cloud, tris = _gpu_mesh(vol, dims, vs, trunc, use_activity)
             assert len(cloud) == len(ref_cloud), name
+            assert np.array_equal(cloud.view(np.uint32), ref_cloud.view(np.uint32)), (name, use_activity)   # point for point, in order
             assert np.array_equal(tris, ref), (name, use_activity)
             assert tris.min() >= 0 and tris.max() < len(cloud)
         if name.startswith("odd"):

@@ -199,13 +199,14 @@ def test_knn_and_warp(orc, M, N):
     assert np.array_equal(p_dev.cpu().numpy()[skipped].view(np.uint32), pts[skipped].view(np.uint32)), "skipped points untouched"
 
 
-@pytest.mark.parametrize("first_nan_normal", [None, 700, 0])
-def test_warp_reference_normal_cursor(orc, first_nan_normal):
+@pytest.mark.parametrize("first_nan_normal,N", [(None, 3000), (700, 3000), (0, 3000), (None, 300_000)],
+                         ids=["None", "700", "0", "None-300000"])              # 300,000 points: more than 1024 blocks to scan
+def test_warp_reference_normal_cursor(orc, first_nan_normal, N):
     """DF_WARP_REF_NORMAL_INDEX: the reference's cursor (warp_field.cpp:182-194) pairs the j-th non-NaN point with normal j and stalls
     for good at the first NaN normal -- with a NaN normal at index 0 (a ray-cast miss at pixel 0) it warps nothing at all"""
     import ctypes as C
     rng = np.random.default_rng(7)
-    M, N = 300, 3000
+    M = 300
     nodes = _random_nodes(rng, M)
     for m in range(M):
         t = rng.normal(scale=0.02, size=3).astype(np.float32)
@@ -237,12 +238,13 @@ def test_warp_reference_normal_cursor(orc, first_nan_normal):
     np.testing.assert_allclose(gn[mn], n_ref[mn], rtol=1e-4, atol=1e-6)
 
 
-@pytest.mark.parametrize("use_grid,max_nodes", [(True, 4096), (False, 4096), (True, 330)])
-def test_extend_field_matches_oracle(orc, use_grid, max_nodes):
+@pytest.mark.parametrize("use_grid,max_nodes,cap", [(True, 4096, 24000), (False, 4096, 24000), (True, 330, 24000), (True, 16384, 330_000)],
+                         ids=["True-4096", "False-4096", "True-330", "True-16384-330000"])    # 275,000 points: past the first 1024 blocks
+def test_extend_field_matches_oracle(orc, use_grid, max_nodes, cap):
     """df_extend_field (SURVEY 8f(3)): same appended nodes, bit for bit, as the oracle's sequential restatement -- the support test is
     the exact nearest-node distance and the subsampling follows cloud order"""
     rng = np.random.default_rng(11)
-    M, P, cap = 300, 20000, 24000
+    M, P = 300, cap * 5 // 6
     nodes = _random_nodes(rng, M)
     nodes[:, :3] *= 0.5                                    # nodes cover the centre of the cloud only
     cloud = np.zeros((cap, 4), np.float32)

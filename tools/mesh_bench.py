@@ -132,8 +132,7 @@ def main():
         torch.cuda.synchronize()
     kernels = {}
     for e in prof.key_averages():
-        for key in ("mesh_count_kernel", "mesh_vertex_base_kernel", "mesh_emit_kernel", "mesh_status_kernel", "extract_scan_local_kernel",
-                    "extract_scan_super_kernel"):
+        for key in ("mesh_count_kernel", "mesh_vertex_base_kernel", "mesh_emit_kernel", "mesh_status_kernel", "scan_block_counts_kernel"):
             if key in e.key:
                 dt = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
                 kernels[key] = round(kernels.get(key, 0.0) + dt / 1e3 / args.reps, 4)
