@@ -140,7 +140,8 @@ PROTOTYPES = {
     "df_kinfu_mesh": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "df_raster_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "df_raster_mesh": (_i, [_vp, _i, _i, _vp, _i, Aff3f, Intr, _i, _i, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _vp, _vp]),
-    "df_kinfu_render": (_i, [_vp, _i, C.POINTER(C.c_float), _vp, _sz, _vp, _sz, _vp, _sz]),
+    "df_mesh_correspond": (_i, [_vp, _sz, _vp, _sz, _vp, _vp, _i, _i, _vp, _i, Aff3f, _i, _i, _vp, _sz, _f, _vp, _sz, _vp, _sz, _vp]),
+    "df_kinfu_render":(_i, [_vp, _i, C.POINTER(C.c_float), _vp, _sz, _vp, _sz, _vp, _sz]),
 }
 
 

@@ -86,7 +86,17 @@ struct KinFu {
     DevMem<int32_t> mesh_tris; size_t mesh_tris_bytes = 0;
     DevMem<float> mesh_moved; size_t mesh_moved_bytes = 0;
     DevMem<void> raster_ws; size_t raster_ws_bytes = 0;
-    float *pinned = nullptr;             // 16 floats: T(12) + ok
+    // DF_KINFU_LIVE_MODEL: the live mesh kept for the next frame (lm_valid): the cloud moved to the ray-cast's voxel convention (lm_src), the
+    // same carried through the warp field (lm_live: points, then normals), lm_N points, lm_T faces in mesh_tris (read through the member at
+    // every use: a re-grow by df_kinfu_mesh / _render re-emits the same faces); lm_ids is the association render's triangle map
+    DevMem<float> lm_src, lm_live; size_t lm_src_bytes = 0, lm_live_bytes = 0;
+    Img lm_ids;
+    int lm_N = 0, lm_T = 0;
+    bool lm_valid = false;
+    bool field_frame = false;            // the last dynamicfusion() warped and solved (a warp field, not a rigid frame)
+    float lm_shift[3] = {0.f, 0.f, 0.f}; // R_vol * (vs/2): extraction puts voxel i at (i + 1/2) vs, integrate and the ray-cast at i vs
+    long long lm_fallbacks = 0; bool lm_fell_back = false;   // frames without a live model; info[12]
+    float *pinned = nullptr;            // 16 floats: T(12) + ok
     std::vector<float> poses;            // 12 floats per pose
     int frame_counter = 0, resets = 0, last_ok = 1, launches = 0;
     // df_kinfu_set_overrides (lock-step parity hook): one-shot replacements for the NEXT frame
@@ -244,6 +254,7 @@ int do_reset(KinFu &k)
     if (k.frame_counter) { printf("Reset\n"); ++k.resets; }          // kinfu.cpp:198-199
     k.frame_counter = 0;
     k.M = 0;                                                         // warp_->clear(), kinfu.cpp:206: the next first frame re-initialises the field
+    k.lm_valid = false;
     k.poses.clear();
     k.poses.resize(12);
     dfh_aff_identity(k.poses.data());
@@ -270,6 +281,7 @@ void note_solve_overflow(KinFu &k)
 void begin_frame(KinFu &k)
 {
     k.launches = 0;
+    k.lm_fell_back = false;
     memset(k.stage_mark, 0, sizeof k.stage_mark);
     mark(k, 0);
 }
@@ -467,27 +479,191 @@ int track(KinFu &k, double &t_sync0, double &t_sync1)
     return 0;
 }
 
+// ---- the mesh of the reconstruction: df_kinfu_mesh / df_kinfu_render, and the live model of DF_KINFU_LIVE_MODEL -----------------
+
+// `m` holds at least `need` bytes (its contents are not kept when it grows)
+template <class T> int grow(DevMem<T> &m, size_t &have, size_t need)
+{
+    if (m && have >= need) return 0;
+    DevMem<T> fresh;
+    CK(fresh.alloc(need));
+    m = std::move(fresh);                                              // the old block is freed with `fresh`
+    have = need;
+    return 0;
+}
+
+// completes the last frame's extraction, counts the triangles (df_mesh_count: 7 launches) and reads back the triangle count, the status and
+// the cloud's point count: one host synchronisation.  match: the cloud matches the volume.
+int mesh_count_now(KinFu &k, int &N, int &T, bool &match)
+{
+    cudaStream_t s = k.stream;
+    sync_extract(k);                                                   // the last frame's cloud is complete
+    const df_volume v = vol_of(k);
+    if (!k.mesh_ws) CK(k.mesh_ws.alloc(df_mesh_workspace_bytes(v)));
+    if (!k.mesh_dev) CK(k.mesh_dev.alloc(64));
+    CK(df_mesh_count(v, k.activity, k.cloud_count, k.mesh_ws, k.mesh_dev, k.mesh_dev + 1, s));
+    int counts[3] = {0, 0, 0};                                         // triangles, status, cloud points
+    CK(cudaMemcpyAsync(counts, k.mesh_dev, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(counts + 2, k.cloud_count, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    match = counts[1] == 0;
+    T = counts[0]; N = counts[2];
+    return 0;
+}
+
+// mesh_count_now for df_kinfu_mesh / df_kinfu_render: *N cloud points, *T triangles, or cudaErrorInvalidValue (reason on stderr, prefixed
+// with `who`) when there is no such mesh
+int mesh_size(KinFu &k, int live, const char *who, int &N, int &T)
+{
+    if (live && k.M < 8) {                                             // the loop warps nothing without a field (dynamicfusion(): k.M >= 8)
+        fprintf(stderr, "%s: no live mesh: the warp field has %d nodes (fewer than 8)\n", who, k.M);
+        return (int)cudaErrorInvalidValue;
+    }
+    bool match = false;
+    CK(mesh_count_now(k, N, T, match));
+    if (!match) {
+        fprintf(stderr, "%s: the extracted cloud (%d points) does not match the volume: truncated at cloud_capacity (%d), or not "
+                        "extracted since the volume last changed\n", who, N, k.p.cloud_capacity);
+        return (int)cudaErrorInvalidValue;
+    }
+    return 0;
+}
+
+// after mesh_size: the T triangles into k.mesh_tris and the vertex buffer (float4 points and, when `nrm` is not null, normals of the N cloud
+// points): the cloud itself, or for `live` copies of it carried through the warp field by the frame loop's own df_warp call (kinfu.cpp:385).
+// The live copy includes the normals even when the caller wants none: df_warp moves only points whose normal is a number, and it writes
+// the warped normal in place, so without the copy the points would differ from df_kinfu_mesh's and the cloud's normals would be overwritten.
+int mesh_build(KinFu &k, int live, int N, int T, const float *&pts, const float **nrm)
+{
+    cudaStream_t s = k.stream;
+    CK(grow(k.mesh_tris, k.mesh_tris_bytes, (size_t)T * 12));
+    CK(df_mesh_emit(vol_of(k), k.activity, k.mesh_ws, k.mesh_tris, T, s));
+    pts = k.cloud;
+    if (nrm) *nrm = k.cloud_nrm;
+    if (live) {
+        CK(grow(k.mesh_moved, k.mesh_moved_bytes, (size_t)N * 32));
+        float *mp = k.mesh_moved, *mn = mp + (size_t)N * 4;
+        CK(cudaMemcpyAsync(mp, k.cloud, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(mn, k.cloud_nrm, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
+        df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);
+        if (N > 0) CK(df_warp(k.nodes, k.M, k.node_grid, mp, mn, N, 4, ident, 0, nullptr, nullptr, s));
+        pts = mp;
+        if (nrm) *nrm = mn;
+    }
+    return 0;
+}
+
+// DF_KINFU_LIVE_MODEL: p - shift for every cloud point (w kept), written twice: the association's source vertices and the copy df_warp carries
+// into the live frame
+__global__ void __launch_bounds__(256) shift_points_kernel(const float4 *cloud, int n, float sx, float sy, float sz, float4 *src, float4 *live)
+{
+    DF_PDL_ENTRY();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 p = cloud[i];
+    const float4 o = make_float4(p.x - sx, p.y - sy, p.z - sz, p.w);
+    src[i] = o;
+    live[i] = o;
+}
+
+bool live_model_on(const KinFu &k) { return (k.p.flags & DF_KINFU_LIVE_MODEL) != 0; }
+
+// a frame whose live mesh could not be built tracks and solves against the ray-casts; counted once per frame (get_info[12])
+void note_live_model_fallback(KinFu &k, int cloud_points)
+{
+    if (k.lm_fell_back) return;
+    k.lm_fell_back = true;
+    if (k.lm_fallbacks++ == 0)
+        fprintf(stderr, "df_kinfu: no live model: the extracted cloud (%d points) does not match the volume (truncated at cloud_capacity = %d); "
+                        "frames like this one track and solve against the ray-casts (df_kinfu_get_info[12] counts them)\n",
+                cloud_points, k.p.cloud_capacity);
+}
+
+// the live mesh of the current state into lm_src / lm_live / mesh_tris (k.lm_valid), or a fallback when the cloud does not match the volume
+int build_live_mesh(KinFu &k)
+{
+    cudaStream_t s = k.stream;
+    k.lm_valid = false;
+    int N = 0, T = 0;
+    bool match = false;
+    CK(mesh_count_now(k, N, T, match));
+    k.launches += 7;
+    if (!match) {
+        note_live_model_fallback(k, N);
+        return 0;
+    }
+    const float *unused;
+    CK(mesh_build(k, 0, N, T, unused, nullptr));                       // the faces, shared with df_kinfu_mesh: the same state emits the same faces
+    ++k.launches;
+    CK(grow(k.lm_src, k.lm_src_bytes, (size_t)N * 16));
+    CK(grow(k.lm_live, k.lm_live_bytes, (size_t)N * 32));
+    float *live_pts = k.lm_live, *live_nrm = live_pts + (size_t)N * 4;
+    CK(cudaMemcpyAsync(live_nrm, k.cloud_nrm, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
+    if (N > 0) {
+        launch_pdl(shift_points_kernel, dim3(div_up(N, 256)), dim3(256), 0, s, (const float4 *)k.cloud.p, N, k.lm_shift[0], k.lm_shift[1],
+                   k.lm_shift[2], (float4 *)k.lm_src.p, (float4 *)live_pts);
+        df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);
+        CK(df_warp(k.nodes, k.M, k.node_grid, live_pts, live_nrm, N, 4, ident, 0, nullptr, nullptr, s));   // as mesh_build(live)
+        k.launches += 2;
+    }
+    k.lm_N = N; k.lm_T = T; k.lm_valid = true;
+    return 0;
+}
+
+// df_raster_mesh of the kept live mesh seen through world2cam
+int raster_live_mesh(KinFu &k, const float *world2cam, int32_t *ids, size_t ids_pitch, Img &pts, Img &nrm)
+{
+    const df_kinfu_params &p = k.p;
+    CK(grow(k.raster_ws, k.raster_ws_bytes, df_raster_workspace_bytes(k.lm_N, k.lm_T, p.cols, p.rows)));
+    CK(df_raster_mesh(k.lm_live, k.lm_N, 4, k.mesh_tris, k.lm_T, to_aff(world2cam), p.intr, p.cols, p.rows, ids, ids_pitch, (float *)pts.ptr,
+                      pts.pitch, (float *)nrm.ptr, nrm.pitch, nullptr, k.raster_ws, k.stream));
+    k.launches += 2 + (k.lm_N > 0) + 2 * (k.lm_T > 0);                 // clear, vertex, triangle + large, resolve
+    return 0;
+}
+
 // ---- KinFu::dynamicfusion, kinfu.cpp:344-400, at the latest pose ---------------------------------------------------
-// depth: the frame's bilateral-filtered depth, modified in place by project-and-remove; live_pts: its level-0 vertex map.
+// depth: the frame's bilateral-filtered depth, modified in place by project-and-remove; live_pts: its level-0 vertex map; prev_pose: the
+// pose of the frame the kept live mesh was built in (DF_KINFU_LIVE_MODEL).
 // Without a warp field (DF_KINFU_RIGID_ONLY, or fewer than 8 nodes) the frame is integrated rigidly: the plain KinFu (Nerei) loop.
-int dynamicfusion(KinFu &k, const Img &depth, const Img &live_pts)
+int dynamicfusion(KinFu &k, const Img &depth, const Img &live_pts, const float *prev_pose)
 {
     const df_kinfu_params &p = k.p;
     cudaStream_t s = k.stream;
     const float *cam_pose = &k.poses[k.poses.size() - 12];
+    k.field_frame = false;
     if ((p.flags & DF_KINFU_RIGID_ONLY) || k.M < 8) {
+        k.lm_valid = false;
         mark(k, 3); mark(k, 4); mark(k, 5); mark(k, 6); mark(k, 7);
         CK(integrate_rigid(k, cam_pose));
         mark(k, 8); mark(k, 9);
         return 0;
     }
+    k.field_frame = true;
     const int npix = p.cols * p.rows;
-    CK(raycast_model(k, cam_pose, k.canon_visible, k.canon_nrm));     // tsdf().raycast(camera_pose, ...), :351 (camera frame)
     float inv_pose[12];
     dfh_aff_inv(cam_pose, inv_pose);
-    launch_pdl(to_canonical_kernel, dim3(div_up(npix, 256)), dim3(256), 0, s, (const float4 *)k.canon_visible.ptr, make_aff(to_aff(inv_pose)),
-                                                           (float4 *)k.canon.ptr, (float4 *)k.canon_visible.ptr, npix);
-    ++k.launches;
+    if (live_model_on(k) && !k.lm_valid) CK(build_live_mesh(k));      // first frame after create, reset or load: the same bits as kept
+    if (live_model_on(k) && k.lm_valid) {
+        // model-to-frame association: the kept live mesh (camera frame of prev_pose) seen from this frame's camera, each pixel paired with
+        // the canonical surface point drawn there; canonical points are model coordinates
+        float inv_prev[12], cam2model[12], world2cam[12];
+        dfh_aff_inv(prev_pose, inv_prev);
+        dfh_aff_mul(inv_prev, cam_pose, cam2model);
+        dfh_aff_inv(cam2model, world2cam);
+        CK(raster_live_mesh(k, world2cam, (int32_t *)k.lm_ids.ptr, k.lm_ids.pitch, k.canon_visible, k.canon_nrm));
+        CK(df_mesh_correspond((const int32_t *)k.lm_ids.ptr, k.lm_ids.pitch, (const float *)k.canon_visible.ptr, k.canon_visible.pitch, k.lm_live,
+                              k.lm_src, k.lm_N, 4, k.mesh_tris, k.lm_T, to_aff(world2cam), p.cols, p.rows, (const float *)live_pts.ptr,
+                              live_pts.pitch, p.icp_dist_thres, (float *)k.canon.ptr, k.canon.pitch, (float *)k.canon_nrm.ptr, k.canon_nrm.pitch, s));
+        ++k.launches;
+        CK(cudaMemcpy2DAsync(k.canon_visible.ptr, k.canon_visible.pitch, k.canon.ptr, k.canon.pitch, (size_t)p.cols * 16, p.rows,
+                             cudaMemcpyDeviceToDevice, s));
+    } else {
+        CK(raycast_model(k, cam_pose, k.canon_visible, k.canon_nrm));     // tsdf().raycast(camera_pose, ...), :351 (camera frame)
+        launch_pdl(to_canonical_kernel, dim3(div_up(npix, 256)), dim3(256), 0, s, (const float4 *)k.canon_visible.ptr, make_aff(to_aff(inv_pose)),
+                                                               (float4 *)k.canon.ptr, (float4 *)k.canon_visible.ptr, npix);
+        ++k.launches;
+    }
+    k.lm_valid = false;                                                // the frame changes the state the mesh was built from
     mark(k, 3);
     df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);    // warp_to_live_ stays identity (never set)
     CK(df_warp(k.nodes, k.M, k.node_grid, (float *)k.canon.ptr, (float *)k.canon_nrm.ptr, npix, 4, ident, DF_WARP_IMAGE_COLS(p.cols), nullptr, nullptr, s));   // :385
@@ -548,7 +724,8 @@ int dynamicfusion(KinFu &k, const Img &depth, const Img &live_pts)
         CK(integrate_rigid(k, cam_pose));
     }
     mark(k, 8);
-    CK(extract_cloud(k, (p.flags & DF_KINFU_EXTEND_FIELD) != 0));     // compute_points / compute_normals, :398-399
+    // compute_points / compute_normals, :398-399; the field extension and the live mesh (raycast_next) read the cloud right away
+    CK(extract_cloud(k, (p.flags & DF_KINFU_EXTEND_FIELD) != 0 || live_model_on(k)));
     CK(extend_field(k));
     mark(k, 9);
     return 0;
@@ -559,6 +736,14 @@ int raycast_next(KinFu &k)
 {
     const df_kinfu_params &p = k.p;
     cudaStream_t s = k.stream;
+    if (live_model_on(k) && k.field_frame) CK(build_live_mesh(k));
+    if (k.lm_valid) {
+        // DF_KINFU_LIVE_MODEL: the live mesh is in this camera's frame; it is kept for the next frame's association
+        float id12[12], world2cam[12];
+        dfh_aff_identity(id12);
+        dfh_aff_inv(id12, world2cam);
+        CK(raster_live_mesh(k, world2cam, nullptr, 0, k.prev_pts[0], k.prev_nrm[0]));
+    } else
     CK(raycast_model(k, &k.poses[k.poses.size() - 12], k.prev_pts[0], k.prev_nrm[0]));
     if (p.flags & DF_KINFU_USE_DEPTH) {
         // TsdfVolume::raycast(pose, intr, Depth&, Normals&) (tsdf_volume.cu:273-339,441-456) = the same march storing ushort(vertex.z * 1000),
@@ -593,7 +778,7 @@ int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool &fused
     if (k.frame_counter == 0) return first_frame(k);
     CK(track(k, t_sync0, t_sync1));
     if (k.frame_counter == 0) return 0;                                // tracking lost: the object was reset
-    CK(dynamicfusion(k, k.cur_depth[0], k.cur_pts[0]));
+    CK(dynamicfusion(k, k.cur_depth[0], k.cur_pts[0], &k.poses[k.poses.size() - 24]));
     CK(raycast_next(k));
     ++k.frame_counter;
     const double t_end = now_us();
@@ -651,6 +836,8 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         if (ud && atoi(ud) != 0) k->p.flags |= DF_KINFU_USE_DEPTH;
         const char *f2e = getenv("DF_KINFU_F2_SOLVE");
         if (f2e && atoi(f2e) != 0) k->p.flags |= DF_KINFU_F2_SOLVE;
+        const char *lm = getenv("DF_KINFU_LIVE_MODEL");
+        if (lm && atoi(lm) != 0) k->p.flags |= DF_KINFU_LIVE_MODEL;
         const char *rb = getenv("DF_RAYCAST_BRICKS");
         if (rb && atoi(rb) == 0) k->raycast_bricks = false;
         const char *w = getenv("DF_FUSION_WEIGHT_SCALE");
@@ -664,6 +851,10 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
     float vmax = 0.f;
     for (int d = 0; d < 3; ++d) { k->voxel_size[d] = p.volume_size[d] / p.volume_dims[d]; vmax = vmax > k->voxel_size[d] ? vmax : k->voxel_size[d]; }
     k->trunc_dist = p.tsdf_trunc_dist > 2.1f * vmax ? p.tsdf_trunc_dist : 2.1f * vmax;   // setTruncDist, tsdf_volume.cpp:68-73
+    {
+        const float h[3] = {k->voxel_size[0] / 2.f, k->voxel_size[1] / 2.f, k->voxel_size[2] / 2.f};
+        for (int r = 0; r < 3; ++r) k->lm_shift[r] = k->vol_pose[3 * r] * h[0] + k->vol_pose[3 * r + 1] * h[1] + k->vol_pose[3 * r + 2] * h[2];
+    }
     const size_t nvox = (size_t)p.volume_dims[0] * p.volume_dims[1] * p.volume_dims[2];
     bool ok = k->volume.alloc(nvox * 4) == cudaSuccess;
     ok = ok && alloc_img(k->depth_in, p.rows, p.cols, 2) == 0 && alloc_img(k->dists, p.rows, p.cols, 2) == 0;
@@ -676,6 +867,7 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
     }
     ok = ok && alloc_img(k->canon, p.rows, p.cols, 16) == 0 && alloc_img(k->canon_nrm, p.rows, p.cols, 16) == 0 &&
          alloc_img(k->canon_visible, p.rows, p.cols, 16) == 0;
+    if (p.flags & DF_KINFU_LIVE_MODEL) ok = ok && alloc_img(k->lm_ids, p.rows, p.cols, 4) == 0;
     ok = ok && k->cloud.alloc((size_t)p.cloud_capacity * 16) == cudaSuccess && k->cloud_nrm.alloc((size_t)p.cloud_capacity * 16) == cudaSuccess;
     ok = ok && k->cloud_count.alloc(64) == cudaSuccess;
     const int maxM = k->max_nodes_cap;
@@ -783,7 +975,7 @@ extern "C" int df_kinfu_dynamicfusion(void *h, uint16_t *depth_dev, size_t depth
     begin_frame(*k);
     mark(*k, 2);                                                      // no tracking: the latest pose is the frame's
     const Img depth{depth_dev, depth_pitch, k->p.cols, k->p.rows}, live{(void *)live_points_dev, live_pitch, k->p.cols, k->p.rows};
-    const int st = dynamicfusion(*k, depth, live);
+    const int st = dynamicfusion(*k, depth, live, &k->poses[k->poses.size() - 12]);   // the latest pose is also the kept live mesh's
     return st ? -st : 1;
 }
 
@@ -831,9 +1023,9 @@ extern "C" int df_kinfu_get_info(void *h, long long *info, int n)
     cudaStreamSynchronize(k->stream);
     const unsigned long long nu = nu2[0];
     note_solve_overflow(*k);
-    const long long vals[12] = {k->frame_counter, k->M, k->last_cloud, (long long)(k->poses.size() / 12), k->last_ok, k->launches, k->resets,
-                                (long long)st[2], (long long)nu, (long long)st[4], (long long)nu2[1], k->solve_overflows};
-    for (int i = 0; i < n && i < 12; ++i) info[i] = vals[i];
+    const long long vals[13] = {k->frame_counter, k->M, k->last_cloud, (long long)(k->poses.size() / 12), k->last_ok, k->launches, k->resets,
+                                (long long)st[2], (long long)nu, (long long)st[4], (long long)nu2[1], k->solve_overflows, k->lm_fallbacks};
+    for (int i = 0; i < n && i < 13; ++i) info[i] = vals[i];
     return 0;
 }
 
@@ -1176,74 +1368,13 @@ extern "C" int df_kinfu_load(void *h, const void *src_host, size_t bytes)
     k->poses.resize((size_t)L.c.n_poses * 12);
     memcpy(k->poses.data(), b + L.poses, (size_t)L.c.n_poses * 48);
     k->extract_deferred = false; k->extract_pending = false;
+    k->lm_valid = false;                                               // DF_KINFU_LIVE_MODEL: the next frame builds it from the loaded state
     return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // Mesh of the reconstruction (df_kinfu_mesh, df_kinfu_render; dfusion.h): triangles over the extracted cloud; reads the volume, the cloud and
-// the nodes only.  The device sequence is shared: mesh_size, then mesh_build.
-
-// `m` holds at least `need` bytes (its contents are not kept when it grows)
-template <class T> int grow(DevMem<T> &m, size_t &have, size_t need)
-{
-    if (m && have >= need) return 0;
-    DevMem<T> fresh;
-    CK(fresh.alloc(need));
-    m = std::move(fresh);                                              // the old block is freed with `fresh`
-    have = need;
-    return 0;
-}
-
-// completes the last frame's extraction, counts the triangles and checks the cloud against the volume: *N cloud points, *T triangles, or
-// cudaErrorInvalidValue (reason on stderr, prefixed with `who`) when there is no such mesh
-int mesh_size(KinFu &k, int live, const char *who, int &N, int &T)
-{
-    if (live && k.M < 8) {                                             // the loop warps nothing without a field (dynamicfusion(): k.M >= 8)
-        fprintf(stderr, "%s: no live mesh: the warp field has %d nodes (fewer than 8)\n", who, k.M);
-        return (int)cudaErrorInvalidValue;
-    }
-    cudaStream_t s = k.stream;
-    sync_extract(k);                                                   // the last frame's cloud is complete
-    const df_volume v = vol_of(k);
-    if (!k.mesh_ws) CK(k.mesh_ws.alloc(df_mesh_workspace_bytes(v)));
-    if (!k.mesh_dev) CK(k.mesh_dev.alloc(64));
-    CK(df_mesh_count(v, k.activity, k.cloud_count, k.mesh_ws, k.mesh_dev, k.mesh_dev + 1, s));
-    int counts[3] = {0, 0, 0};                                         // triangles, status, cloud points
-    CK(cudaMemcpyAsync(counts, k.mesh_dev, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(counts + 2, k.cloud_count, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    if (counts[1] != 0) {
-        fprintf(stderr, "%s: the extracted cloud (%d points) does not match the volume: truncated at cloud_capacity (%d), or not "
-                        "extracted since the volume last changed\n", who, counts[2], k.p.cloud_capacity);
-        return (int)cudaErrorInvalidValue;
-    }
-    T = counts[0]; N = counts[2];
-    return 0;
-}
-
-// after mesh_size: the T triangles into k.mesh_tris and the vertex buffer (float4 points and, when `nrm` is not null, normals of the N cloud
-// points): the cloud itself, or for `live` copies of it carried through the warp field by the frame loop's own df_warp call (kinfu.cpp:385).
-// The live copy includes the normals even when the caller wants none: df_warp moves only points whose normal is a number, and it writes
-// the warped normal in place, so without the copy the points would differ from df_kinfu_mesh's and the cloud's normals would be overwritten.
-int mesh_build(KinFu &k, int live, int N, int T, const float *&pts, const float **nrm)
-{
-    cudaStream_t s = k.stream;
-    CK(grow(k.mesh_tris, k.mesh_tris_bytes, (size_t)T * 12));
-    CK(df_mesh_emit(vol_of(k), k.activity, k.mesh_ws, k.mesh_tris, T, s));
-    pts = k.cloud;
-    if (nrm) *nrm = k.cloud_nrm;
-    if (live) {
-        CK(grow(k.mesh_moved, k.mesh_moved_bytes, (size_t)N * 32));
-        float *mp = k.mesh_moved, *mn = mp + (size_t)N * 4;
-        CK(cudaMemcpyAsync(mp, k.cloud, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
-        CK(cudaMemcpyAsync(mn, k.cloud_nrm, (size_t)N * 16, cudaMemcpyDeviceToDevice, s));
-        df_aff3f ident; float id12[12]; dfh_aff_identity(id12); ident = to_aff(id12);
-        if (N > 0) CK(df_warp(k.nodes, k.M, k.node_grid, mp, mn, N, 4, ident, 0, nullptr, nullptr, s));
-        pts = mp;
-        if (nrm) *nrm = mn;
-    }
-    return 0;
-}
+// the nodes only.  The device sequence is shared with the frame loop's live model (above): mesh_size, then mesh_build.
 
 extern "C" int df_kinfu_mesh(void *h, int live, float *verts_host, float *normals_host, int32_t *tris_host, int vert_capacity, int tri_capacity,
                              int *n_verts, int *n_tris)

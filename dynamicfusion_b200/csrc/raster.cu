@@ -223,7 +223,77 @@ __global__ void __launch_bounds__(256) raster_resolve_kernel(const unsigned long
     if (tri_ids) row_ptr(tri_ids, tpitch, j)[i] = id;
 }
 
+// df_mesh_correspond: one thread per pixel; the drawn triangle's corners are recomputed exactly as raster_vertex_kernel computes them
+__global__ void __launch_bounds__(256) correspond_kernel(const int32_t *tri_ids, size_t tpitch, const float4 *points, size_t ppitch,
+                                                         const float *verts, const float *src, int n_verts, int vstride, const int32_t *tris,
+                                                         int n_tris, Aff w2c, int cols, int rows, const float4 *target, size_t gpitch,
+                                                         float max_dist, float4 *out_pts, size_t opitch, float4 *out_nrm, size_t npitch)
+{
+    DF_PDL_ENTRY();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y * blockDim.y + threadIdx.y;
+    if (i >= cols || j >= rows) return;
+    const float nanv = qnan();
+    float4 S = make_float4(nanv, nanv, nanv, nanv), N = S;
+    const int id = row_ptr(tri_ids, tpitch, j)[i];
+    if (id >= 0 && id < n_tris) {
+        const int ix[3] = {tris[3 * (size_t)id], tris[3 * (size_t)id + 1], tris[3 * (size_t)id + 2]};
+        bool ok = (unsigned)ix[0] < (unsigned)n_verts && (unsigned)ix[1] < (unsigned)n_verts && (unsigned)ix[2] < (unsigned)n_verts;
+        const float4 P4 = row_ptr(points, ppitch, j)[i];
+        const float3 P = make_float3(P4.x, P4.y, P4.z);
+        if (ok && target) {
+            const float4 T = row_ptr(target, gpitch, j)[i];
+            const float dx = T.x - P.x, dy = T.y - P.y, dz = T.z - P.z;
+            ok = !isnan(T.x) && !isnan(T.y) && !isnan(T.z) && !(dx * dx + dy * dy + dz * dz > max_dist * max_dist);
+        }
+        if (ok) {
+            float3 c[3], s[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const float *v = verts + (size_t)ix[k] * vstride, *w = src + (size_t)ix[k] * vstride;
+                const float x = v[0], y = v[1], z = v[2];
+                c[k] = make_float3(w2c.r0.x * x + w2c.r0.y * y + w2c.r0.z * z + w2c.t.x, w2c.r1.x * x + w2c.r1.y * y + w2c.r1.z * z + w2c.t.y,
+                                   w2c.r2.x * x + w2c.r2.y * y + w2c.r2.z * z + w2c.t.z);
+                s[k] = make_float3(w[0], w[1], w[2]);
+            }
+            const float3 e0 = make_float3(c[1].x - c[0].x, c[1].y - c[0].y, c[1].z - c[0].z);
+            const float3 e1 = make_float3(c[2].x - c[0].x, c[2].y - c[0].y, c[2].z - c[0].z);
+            const float3 q = make_float3(P.x - c[0].x, P.y - c[0].y, P.z - c[0].z);
+            const float d00 = rdot(e0, e0), d01 = rdot(e0, e1), d11 = rdot(e1, e1), d20 = rdot(q, e0), d21 = rdot(q, e1);
+            const float den = d00 * d11 - d01 * d01;
+            if (isfinite(den) && den != 0.f) {
+                const float b1 = (d11 * d20 - d01 * d21) / den, b2 = (d00 * d21 - d01 * d20) / den, b0 = 1.f - b1 - b2;
+                S = make_float4((b0 * s[0].x + b1 * s[1].x) + b2 * s[2].x, (b0 * s[0].y + b1 * s[1].y) + b2 * s[2].y,
+                                (b0 * s[0].z + b1 * s[1].z) + b2 * s[2].z, 0.f);
+                const float3 n = rcross(make_float3(s[1].x - s[0].x, s[1].y - s[0].y, s[1].z - s[0].z),
+                                        make_float3(s[2].x - s[0].x, s[2].y - s[0].y, s[2].z - s[0].z));
+                const float len = sqrtf(rdot(n, n));
+                N = make_float4(n.x / len, n.y / len, n.z / len, 0.f);
+            }
+        }
+    }
+    row_ptr(out_pts, opitch, j)[i] = S;
+    row_ptr(out_nrm, npitch, j)[i] = N;
+}
+
 }  // namespace
+
+extern "C" int df_mesh_correspond(const int32_t *tri_ids, size_t tri_pitch, const float *points, size_t points_pitch, const float *verts,
+                                  const float *src_verts, int n_verts, int vstride, const int32_t *tris, int n_tris, df_aff3f world2cam, int cols,
+                                  int rows, const float *target, size_t target_pitch, float max_dist, float *src_points, size_t src_points_pitch,
+                                  float *src_normals, size_t src_normals_pitch, void *stream)
+{
+    if (n_verts < 0 || n_tris < 0 || (vstride != 3 && vstride != 4) || cols <= 0 || rows <= 0 || cols > DF_RASTER_MAX_DIM ||
+        rows > DF_RASTER_MAX_DIM || !tri_ids || !points || !src_points || !src_normals || (n_verts > 0 && (!verts || !src_verts)) ||
+        (n_tris > 0 && !tris) || tri_pitch < (size_t)cols * 4 || tri_pitch % 4 || points_pitch < (size_t)cols * 16 || points_pitch % 16 ||
+        src_points_pitch < (size_t)cols * 16 || src_points_pitch % 16 || src_normals_pitch < (size_t)cols * 16 || src_normals_pitch % 16 ||
+        (target && (target_pitch < (size_t)cols * 16 || target_pitch % 16)))
+        return (int)cudaErrorInvalidValue;
+    launch_pdl(correspond_kernel, dim3(div_up(cols, 32), div_up(rows, 8)), dim3(32, 8), 0, (cudaStream_t)stream, tri_ids, tri_pitch,
+               (const float4 *)points, points_pitch, verts, src_verts, n_verts, vstride, tris, n_tris, make_aff(world2cam), cols, rows,
+               (const float4 *)target, target_pitch, max_dist, (float4 *)src_points, src_points_pitch, (float4 *)src_normals, src_normals_pitch);
+    DF_LAUNCH_CHECK();
+    return 0;
+}
 
 extern "C" size_t df_raster_workspace_bytes(int n_verts, int n_tris, int cols, int rows)
 {

@@ -21,6 +21,7 @@ EXTEND_FIELD = 16         # DF_KINFU_EXTEND_FIELD: grow the warp field over unsu
 F2_SOLVE = 32             # DF_KINFU_F2_SOLVE: robust 6-DoF data term + regulariser instead of the translation-only solve (SURVEY 8f(2))
 USE_DEPTH = 64            # DF_KINFU_USE_DEPTH: the reference's compile-time USE_DEPTH frame loop (depth-pyramid ICP)
 WARPED_INTEGRATE = 8      # DF_KINFU_WARPED_INTEGRATE: per-voxel warped fusion (SURVEY 8f(1)) instead of the rigid fallback
+LIVE_MODEL = 128          # DF_KINFU_LIVE_MODEL: ICP and the data term's association against the rendered live model, not the canonical ray-casts
 
 
 class KinFuParams:
@@ -95,10 +96,10 @@ class KinFu:
         return a[:9].reshape(3, 3), a[9:]
 
     def info(self) -> dict:
-        v = (C.c_longlong * 12)()
-        self.lib.df_kinfu_get_info(self.h, v, 12)
+        v = (C.c_longlong * 13)()
+        self.lib.df_kinfu_get_info(self.h, v, 13)
         keys = ["frame_counter", "nodes", "cloud_points", "poses", "icp_ok", "launches", "resets", "lm_iters", "n_updated", "pcg_iters",
-                "n_warped", "solve_overflows"]
+                "n_warped", "solve_overflows", "live_model_fallbacks"]
         return dict(zip(keys, [int(x) for x in v]))
 
     def set_overrides(self, bilateral_depth=None, pose=None, nodes=None) -> None:

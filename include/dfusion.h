@@ -219,6 +219,29 @@ int df_raster_mesh(const float *verts, int n_verts, int vstride, const int32_t *
                    int rows, int32_t *tri_ids, size_t tri_pitch, float *points, size_t points_pitch, float *normals, size_t normals_pitch,
                    unsigned long long *stats_dev, void *workspace, void *stream);
 
+/* Per-pixel correspondences on a second vertex set with the same faces (csrc/raster.cu): for a df_raster_mesh view of a mesh (tri_ids and
+ * the drawn points of that call, and its verts / vstride / tris / world2cam), the point of the SOURCE mesh (src_verts: same count, stride and
+ * triangles as verts) at the same barycentric position on the drawn triangle, and that source triangle's face normal.  The frame loop uses
+ * it to pair each pixel of the rendered live model with the canonical surface drawn there (DF_KINFU_LIVE_MODEL).
+ *   Rule (tests/correspond_oracle.c implements it operation for operation; IEEE round-to-nearest, no contraction, evaluated as written):
+ *   c0, c1, c2    the drawn triangle's corners in the camera frame, computed as df_raster_mesh's Camera frame rule; s0, s1, s2 its source
+ *                 corners (xyz of src_verts).
+ *   P             the drawn point (xyz).  e0 = c1 - c0, e1 = c2 - c0, q = P - c0; d00 = dot(e0, e0), d01 = dot(e0, e1), d11 = dot(e1, e1),
+ *                 d20 = dot(q, e0), d21 = dot(q, e1) (dot = x*x' + y*y' + z*z' left to right); den = d00 * d11 - d01 * d01;
+ *                 b1 = (d11 * d20 - d01 * d21) / den, b2 = (d00 * d21 - d01 * d20) / den, b0 = (1 - b1) - b2.
+ *   Output        src_points = ((b0 * s0 + b1 * s1) + b2 * s2, 0) per component; src_normals = (n / sqrt(dot(n, n)), 0) with
+ *                 n = cross(s1 - s0, s2 - s0) in the mesh's order (pointing to free space, like df_raster_mesh's normals).
+ *   No correspondence (four NaNs in both maps): tri id < 0 (or not below n_tris, or a corner index outside [0, n_verts)); den not finite or
+ *                 zero; a target map is given (float4 vertex map, e.g. the frame's) and its vertex at the pixel has a NaN component, or
+ *                 (T - P) has dx*dx + dy*dy + dz*dz > max_dist * max_dist.
+ * target may be NULL (no gate).  cols, rows <= DF_RASTER_MAX_DIM.  Pitches in bytes: points, target, src_points and src_normals at least
+ * cols * 16 and a multiple of 16, tri_ids at least cols * 4 and a multiple of 4 (else cudaErrorInvalidValue, nothing written).  One thread per
+ * pixel, one launch. */
+int df_mesh_correspond(const int32_t *tri_ids, size_t tri_pitch, const float *points, size_t points_pitch, const float *verts,
+                       const float *src_verts, int n_verts, int vstride, const int32_t *tris, int n_tris, df_aff3f world2cam, int cols, int rows,
+                       const float *target, size_t target_pitch, float max_dist, float *src_points, size_t src_points_pitch, float *src_normals,
+                       size_t src_normals_pitch, void *stream);
+
 /* ------------------------------------------------------------------ image processing ----------------------------------------------------- */
 /* device::bilateralFilter (internal.hpp:125, imgproc.cu:11-57) */
 int df_bilateral(const uint16_t *src, size_t src_pitch, int cols, int rows, uint16_t *dst, size_t dst_pitch,
@@ -435,6 +458,16 @@ typedef struct df_kinfu_params {
 #define DF_KINFU_EXTEND_FIELD 16    /* SURVEY 8f(3): after every extraction the warp field is extended (df_extend_field, radius = extend_radius, step = node_step,
                                       up to max_nodes) and the node grid rebuilt; costs one 4-byte read-back per frame.  Environment: DF_KINFU_EXTEND_FIELD=1,
                                       DF_EXTEND_RADIUS. */
+#define DF_KINFU_LIVE_MODEL 128     /* track and solve against the rendered live model (DynamicFusion's model-to-frame association) instead of ray-casts of the
+                                      undeformed canonical volume.  At the end of every frame fused with a warp field, the frame's mesh (df_mesh_count / _emit
+                                      over the cloud, the cloud moved by -R_vol * (vs/2) to the ray-cast's voxel convention, carried through the field by
+                                      df_warp) is rasterised at the identity camera into the previous-frame maps that the next ICP tracks against.  The next
+                                      frame renders that mesh from the ICP increment poses[-2]^-1 * poses[-1] and takes its canonical points from
+                                      df_mesh_correspond (source = the moved, unwarped cloud; target = the frame's vertex map, max_dist = icp_dist_thres): they
+                                      are model coordinates, not pose^-1 * p_camera.  Rigid frames keep the ray-casts; a mesh that cannot be built (cloud
+                                      truncated at cloud_capacity) falls back to them for the frame (df_kinfu_get_info[12], reported once on stderr).  The
+                                      extraction then runs on the main stream, and the triangle count costs one host read-back per frame.  Environment:
+                                      DF_KINFU_LIVE_MODEL=1. */
 
 /* which = 0: KinFuParams::default_params_dynamicfusion (kinfu.cpp:14-49); 1: default_params (kinfu.cpp:55-89) */
 void df_kinfu_default_params(df_kinfu_params *p, int which);
@@ -469,7 +502,8 @@ int df_kinfu_get_pose(void *kinfu, int time, float *pose12_host);
  * [5] kernels launched in the last frame, [6] resets so far, [7] solver LM iterations (last frame),
  * [8] voxels written by the last integrate (DF_KINFU_STAGE_TIMING only), [9] solver PCG iterations (last frame),
  * [10] voxels carried through the warp field by the last df_integrate_warped (DF_KINFU_WARPED_INTEGRATE + STAGE_TIMING),
- * [11] frames whose warp solve was skipped because a normal-matrix row overflowed (df_solve_data_term: stats[5]); also reported on stderr */
+ * [11] frames whose warp solve was skipped because a normal-matrix row overflowed (df_solve_data_term: stats[5]); also reported on stderr,
+ * [12] DF_KINFU_LIVE_MODEL: frames that fell back to the ray-casts because the live mesh could not be built (the first one reported on stderr) */
 int df_kinfu_get_info(void *kinfu, long long *info_host, int n);
 /* device buffers of the current state: 0 volume(u32), 1 dists, 2 curr depth L0, 3 curr points L0, 4 curr normals L0,
  * 5 prev points L0, 6 prev normals L0, 7 canonical (after 2nd warp), 8 canonical normals, 9 extracted cloud,
