@@ -110,6 +110,7 @@ PROTOTYPES = {
     "df_integrate_warped": (_i, [Volume, _vp, _sz, _i, _i, Aff3f, Aff3f, Intr, _vp, _i, _vp, _f, _vp, _vp, _vp, _vp]),
     "df_solve_workspace_bytes": (_sz, [_i, _i]),
     "df_solve_knn_buffers": (_i, [_vp, _i, _i, C.POINTER(_vp), C.POINTER(_vp)]),
+    "df_solve_normal_system": (_i, [_vp, _i, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp)]),
     "df_solve_data_term": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "df_solve_f2_workspace_bytes": (_sz, [_i, _i, _i]),
     "df_solve_f2": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, C.POINTER(F2Params), _vp, _vp, _vp]),

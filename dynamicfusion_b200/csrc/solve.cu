@@ -201,7 +201,9 @@ __global__ void __launch_bounds__(256) solve_blockscan_kernel(SolveWs ws, int M)
 // (node, block); the block's cursors live in a small shared-memory hash and its warps take their turns one after the other, so every
 // entry's position is a pure function of the data.  (A first version sorted the block's 2,048 (node, entry) pairs with a bitonic
 // network, which cost more than this.)
-constexpr int FILL_HASH = 1024;                                    // >= distinct nodes a block of 256 vertices can touch (<= 2,048 entries; typically ~30)
+// >= distinct nodes a block of 256 vertices can touch: 256 x 8 = 2,048 entries (typically ~30 nodes for an image, but a flat list in no
+// spatial order touches ~1,300 of 2,000 nodes).  A smaller table could overflow, and an overflowing block writes none of its entries.
+constexpr int FILL_HASH = 2048;
 __global__ void __launch_bounds__(256) solve_fill_kernel(SolveWs ws, int N, int only_if_flag, int cols)
 {
     DF_PDL_ENTRY();
@@ -776,10 +778,12 @@ __global__ void __launch_bounds__(LM_THREADS) solve_lm_kernel(float *nodes, int 
     }
     __syncthreads();
     // cost0 = 0.5|b|^2 - x.gb + 0.5 x^T A x
-    double c0 = 0.0, nvalid = 0.0;
+    double c0 = 0.0, nvalid = 0.0, nnz = 0.0;
     for (int i = tid; i < ws.prepare_blocks * (PREPARE_THREADS / 32); i += LM_THREADS) { c0 += ws.c0_partials[2 * i]; nvalid += ws.c0_partials[2 * i + 1]; }
+    for (int n = tid; n < M; n += LM_THREADS) nnz += (double)ws.rownnz[n];
     c0 = block_sum(c0, red);
     nvalid = block_sum(nvalid, red);
+    nnz = block_sum(nnz, red);
     spmv(ws, M, x, Ap);
     double t0 = 0.0;
     for (int i = tid; i < M3; i += LM_THREADS) t0 += x[i] * (0.5 * Ap[i] - ws.gb[i]);
@@ -881,6 +885,7 @@ __global__ void __launch_bounds__(LM_THREADS) solve_lm_kernel(float *nodes, int 
     }
     if (tid == 0 && stats) {
         stats[0] = cost0; stats[1] = cost; stats[2] = (double)it; stats[3] = nvalid; stats[4] = (double)pcg_total; stats[5] = (double)ws.flags[0];
+        stats[6] = nnz; stats[7] = (ws.flags[3] && !ws.flags[2]) ? -1.5 : -2.0;   // -2: solved by this kernel; -1.5: matrix from the tile records
     }
 }
 
@@ -1855,6 +1860,17 @@ extern "C" int df_solve_knn_buffers(void *workspace, int M, int N, int32_t **idx
     char *base = (char *)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
     layout(ws, base, M, N);
     *idx = ws.idx; *w = ws.w;
+    return 0;
+}
+
+// The assembly kernels (solve_rows / solve_rows_tiles) write these arrays; the LM kernels (one-block, v5, v6) only read them, so after a
+// solve they hold the system the LM iteration was given.
+extern "C" int df_solve_normal_system(void *workspace, int M, int N, int32_t **rownnz, int32_t **col, double **val, double **gb, double **diag)
+{
+    SolveWs ws;
+    char *base = (char *)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    layout(ws, base, M, N);
+    *rownnz = ws.rownnz; *col = ws.col; *val = ws.val; *gb = ws.gb; *diag = ws.diag;
     return 0;
 }
 

@@ -475,8 +475,9 @@ int df_integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_pitch
  * -> Opt LM/PCG on kfusion/solvers/dynamicfusion.t: translation-only data term solved on the device; node
  * translations are updated in place (encodeTranslation, CombinedSolver.h:189-197).
  * params: nonlinear (LM) iterations, linear (PCG) iterations; stats_dev (device, 8 doubles): initial cost, final cost,
- * LM iterations run, valid rows, PCG iterations run, row-overflow flag, [6] non-zeros of the normal matrix, [7] diagnostics (>= 0: solved
- * by the one-exchange cluster kernel, value = halo columns exchanged per PCG step; < 0: by its fallback; fraction .5: matrix assembled from tile records).  If a node's row of the normal matrix couples to more columns
+ * LM iterations run, valid rows, PCG iterations run, row-overflow flag, [6] non-zeros of the normal matrix, [7] which LM kernel solved it
+ * (>= 0: the one-exchange cluster kernel, value = halo columns exchanged per PCG step; -1: the two-exchange cluster kernel, its fallback;
+ * -2: the one-block kernel, for systems no cluster holds; fraction .5 (0.5, -0.5, -1.5): matrix assembled from tile records).  If a node's row of the normal matrix couples to more columns
  * than the kernels store (512), the flag is raised and the solve leaves the node translations UNCHANGED (0 LM iterations) rather than
  * solving a truncated, asymmetric system; callers must look at stats[5] (the frame loop reports it through df_kinfu_get_info[11] and on
  * stderr, the C++ mirror prints an error).  workspace from df_solve_workspace_bytes(M, N).
@@ -486,6 +487,12 @@ size_t df_solve_workspace_bytes(int M, int N);
  * `canon`, inside `workspace` -- valid until the workspace is reused; lets the following warp of the same vertices skip its
  * k-NN pass (DF_WARP_REUSE_KNN) */
 int df_solve_knn_buffers(void *workspace, int M, int N, int32_t **idx, float **w);
+/* after df_solve_data_term: the normal system A x = gb the LM iteration was given, as device pointers into `workspace` (A = W^T W,
+ * gb = W^T b of the data term).  A is stored ELL, column-major with stride M: row i has rownnz[i] entries, entry e at col[e * M + i] /
+ * val[e * M + i] (e < 512), columns ascending; gb is axis-major [3 * M] (gb[a * M + i]); diag [M] = A_ii (0 for a row without support).
+ * Only the assembly kernels write these arrays (the LM kernels read them), so they stay valid until the workspace is reused.  Not
+ * meaningful when stats[5] reported a row overflow. */
+int df_solve_normal_system(void *workspace, int M, int N, int32_t **rownnz, int32_t **col, double **val, double **gb, double **diag);
 #define DF_SOLVE_REF_GRAPH_QUIRK 1
 /* flags bits 8..23: the vertices are an image of that many columns (N = cols * rows, row-major, cols % 16 == 0, rows % 8 == 0): lets the
  * assembly of the normal matrix work tile by tile (16 x 8 pixels share a dozen nodes) instead of entry by entry.  Same result up to the
