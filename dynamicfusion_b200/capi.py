@@ -99,6 +99,7 @@ PROTOTYPES = {
     "df_icp_accumulate_depth": (_i, [_vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz, _i, _i, Intr, Aff3f, _f, _f, _vp, _vp]),
     "df_icp_estimate_depth": (_i, [C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i), C.POINTER(_i),
                                    C.POINTER(_sz), C.POINTER(_sz), _i, C.POINTER(_i), Intr, _f, _f, _vp, _vp, _vp, _vp]),
+    "df_icp_solve_step": (_i, [_vp, _i, _vp, _vp, _vp]),
     "df_knn8": (_i, [_vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "df_node_grid_bytes": (_sz, [_i]),
     "df_build_node_grid": (_i, [_vp, _i, _vp, _vp]),

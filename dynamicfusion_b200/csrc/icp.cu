@@ -219,7 +219,8 @@ __device__ double det6_dev(const double *Ain)
 // The tail is the serial part of every one of a frame's 19 ICP iterations, so its LATENCY is what counts: a double sqrt or division is
 // a ~250-cycle dependent chain, and the textbook form needs 6 + 18 of them.  Here each pivot costs one rsqrt (L_jj = d * rsqrt(d),
 // 1 / L_jj = rsqrt(d)) and the substitutions multiply by the stored inverses: ~1.5 k cycles instead of ~6.5 k.  The solution moves by
-// a few double ulps (the pose is cast to float right after; parity bar 1e-5, tests/test_stages_gpu.py::test_icp_*).
+// a few double ulps (the pose is cast to float right after).  tests/test_icp_reference_gpu.py holds every step, on this path and the
+// fallback's, to the float64 eigen-decomposition step of tests/icp_reference.py: a few float ulps plus 8 kappa_eff eps64 |r| (1 + |t|).
 __device__ __forceinline__ bool chol6_solve(const double (&A)[36], const double (&b)[6], double (&x)[6], double *det)
 {
     double L[36], inv[6];
@@ -515,4 +516,13 @@ extern "C" int df_icp_estimate_depth(const unsigned short *const *dcurr, const f
     if (!dcurr || !dprev) return (int)cudaErrorInvalidValue;
     return icp_estimate_impl(nullptr, dcurr, ncurr, nullptr, dprev, nprev, cols, rows, normals_pitch, depth_pitch, levels, iters, intr,
                              dist_thres, angle_thres, T_dev, ok_dev, scratch, (cudaStream_t)stream);
+}
+
+extern "C" int df_icp_solve_step(const double *partials, int nblocks, float *T, int *ok, void *stream)
+{
+    if ((size_t)partials & 15) return (int)cudaErrorMisalignedAddress;
+    if (nblocks < 1) return (int)cudaErrorInvalidValue;
+    launch_pdl(icp_solve_kernel, dim3(1), dim3(256), 0, (cudaStream_t)stream, partials, nblocks, T, ok, (const float *)T, (const int *)ok);
+    DF_LAUNCH_CHECK();
+    return 0;
 }

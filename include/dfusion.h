@@ -415,6 +415,14 @@ int df_icp_estimate_depth(const unsigned short *const *dcurr, const float *const
                           const size_t *normals_pitch, int levels, const int *iters, df_intr intr, float dist_thres,
                           float angle_thres, float *T_dev, int *ok_dev, double *scratch, void *stream);
 
+/* Test hook: one solve step of df_icp_estimate on a caller's table of per-block partial sums, as the iteration loop runs it after each
+ * accumulate pass.  partials: nblocks rows of 27 doubles in device memory, 16-byte aligned; when 27 * nblocks is odd the table is
+ * followed by one more (slack) double that is read and ignored.  The rows are summed in the loop's fixed order, rounded to float,
+ * solved (Cholesky, else the |det| < 1e-15 gate and the eigen pseudo-inverse) and T (device, 12 floats) <- Tinc * T in place.
+ * *ok (device int) must be non-zero on entry, else the step is skipped as after a failed iteration; it is set to 0 when the step
+ * fails, and T is then left unchanged. */
+int df_icp_solve_step(const double *partials, int nblocks, float *T, int *ok, void *stream);
+
 /* ------------------------------------------------------------------ warp field ------------------------------------------------------------ */
 /* deformation_node (warp_field.hpp:35-40) as 12 floats: vertex[3], rotation quat (w,x,y,z), dual/translation quat
  * (w,x,y,z) = 0.5*t*r (dual_quaternion.hpp:59-63), weight. */

@@ -45,6 +45,8 @@ def load() -> C.CDLL:
         _lib.orc_integrate_warped.restype = C.c_longlong
         _lib.orc_icp_accumulate.restype = C.c_longlong
         _lib.orc_icp_accumulate_depth.restype = C.c_longlong
+        _lib.orc_icp_rows.restype = C.c_longlong
+        _lib.orc_icp_rows_depth.restype = C.c_longlong
         _lib.orc_float2half_rn.restype = C.c_uint16
         _lib.orc_float2half_rn.argtypes = [C.c_float]
         _lib.orc_half2float.restype = C.c_float
@@ -286,6 +288,30 @@ def icp_accumulate_depth(dcurr, ncurr, dprev, nprev, K_level, T, dist2, min_cos)
                                         _p(nprev), C.c_size_t(cols * 16), cols, rows, intr(*K_level), aff(*T), C.c_float(dist2),
                                         C.c_float(min_cos), _p(out))
     return out, int(n)
+
+
+def icp_rows(vcurr, ncurr, vprev, nprev, K_level, T, dist2, min_cos):
+    """the per-pixel rule of icp_accumulate: rows [rows, cols, 7] float32 (NaN where rejected), match [rows, cols] int32 (linear
+    index of the matched previous pixel, -1 where rejected) and the inlier count"""
+    rows, cols = vcurr.shape[:2]
+    out = np.empty((rows, cols, 7), np.float32)
+    match = np.empty((rows, cols), np.int32)
+    n = load().orc_icp_rows(_p(vcurr), C.c_size_t(cols * 16), _p(ncurr), C.c_size_t(cols * 16), _p(vprev), C.c_size_t(cols * 16),
+                            _p(nprev), C.c_size_t(cols * 16), cols, rows, intr(*K_level), aff(*T), C.c_float(dist2), C.c_float(min_cos),
+                            _p(out), _p(match))
+    return out, match, int(n)
+
+
+def icp_rows_depth(dcurr, ncurr, dprev, nprev, K_level, T, dist2, min_cos):
+    """icp_rows for the USE_DEPTH variant"""
+    rows, cols = dcurr.shape[:2]
+    dcurr, dprev = np.ascontiguousarray(dcurr, np.uint16), np.ascontiguousarray(dprev, np.uint16)
+    out = np.empty((rows, cols, 7), np.float32)
+    match = np.empty((rows, cols), np.int32)
+    n = load().orc_icp_rows_depth(_p(dcurr), C.c_size_t(cols * 2), _p(ncurr), C.c_size_t(cols * 16), _p(dprev), C.c_size_t(cols * 2),
+                                  _p(nprev), C.c_size_t(cols * 16), cols, rows, intr(*K_level), aff(*T), C.c_float(dist2),
+                                  C.c_float(min_cos), _p(out), _p(match))
+    return out, match, int(n)
 
 
 def icp_estimate_depth(dcurr, ncurr, dprev, nprev, iters, K, dist_thres, angle_thres):

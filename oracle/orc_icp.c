@@ -6,10 +6,123 @@
 #include "orc_common.h"
 #include <float.h>
 
-/* ComputeIcpHelper::find_coresp (points variant), proj_icp.cu:80-108; row build :359-368.
- * Products row_i*row_j are formed in float (proj_icp.cu:137-345), summed here in double: the reference's
- * float tree-sum order is launch-geometry dependent, so parity on the 27 sums is 1e-5 relative.
- * Returns the number of inlier correspondences. */
+/* ComputeIcpHelper::find_coresp (points variant), proj_icp.cu:80-108; row build :359-368.  The rule for one pixel (x, y):
+ * returns the linear index v * cols + u of the matched previous pixel and writes the 7-float row, or returns -1 when the pixel
+ * is rejected (row untouched). */
+static long long icp_row_points(const float *vcurr, size_t vcpitch, const float *ncurr, size_t ncpitch, const float *vprev, size_t vppitch,
+                                const float *nprev, size_t nppitch, int cols, int rows, orc_intr k, const orc_aff3f *T,
+                                float dist2_thres, float min_cosine, int x, int y, float row[7])
+{
+    const float *vc = orc_row_f4(vcurr, vcpitch, y) + 4 * x;
+    orc_f3 s = f3(vc[0], vc[1], vc[2]);
+    if (isnan(s.x)) return -1;
+    s = orc_aff_mul(T, s);
+    float u = fmaf(k.fx, s.x / s.z, k.cx);
+    float v = fmaf(k.fy, s.y / s.z, k.cy);
+    if (s.z <= 0 || u < 0 || v < 0 || u >= (float)cols || v >= (float)rows) return -1;
+    if (!(u == u) || !(v == v)) return -1;
+    const float *dp = orc_row_f4(vprev, vppitch, (int)v) + 4 * (int)u;
+    orc_f3 d = f3(dp[0], dp[1], dp[2]);
+    if (isnan(d.x)) return -1;
+    orc_f3 df = orc_sub(s, d);
+    float dist2 = orc_dot(df, df);
+    if (dist2 > dist2_thres) return -1;
+    const float *nc = orc_row_f4(ncurr, ncpitch, y) + 4 * x;
+    orc_f3 ns = orc_mat_mul(T->R, f3(nc[0], nc[1], nc[2]));
+    const float *np = orc_row_f4(nprev, nppitch, (int)v) + 4 * (int)u;
+    orc_f3 nd = f3(np[0], np[1], np[2]);
+    float cosine = fabsf(orc_dot(ns, nd));
+    if (!(cosine >= min_cosine)) { if (cosine < min_cosine) return -1; }   /* NaN cosine passes, as in the reference */
+    orc_f3 c = orc_cross(s, nd);
+    row[0] = c.x; row[1] = c.y; row[2] = c.z; row[3] = nd.x; row[4] = nd.y; row[5] = nd.z;
+    row[6] = orc_dot(nd, orc_sub(d, s));
+    return (long long)(int)v * cols + (int)u;
+}
+
+/* ComputeIcpHelper::find_coresp, USE_DEPTH variant (proj_icp.cu:47-78; compiled in when internal.hpp:6 defines USE_DEPTH):
+ * the source point is the current depth pixel (u16 millimetres) re-projected with finv = 1/f (reproj, proj_icp.cu:39-45), the
+ * destination is the previous depth map point-sampled at the projection (texture<ushort> dprev_tex, cudaFilterModePoint) and
+ * re-projected at the fractional coordinates; normals as in the points variant.  Same return value and row as icp_row_points. */
+static long long icp_row_depth(const unsigned short *dcurr, size_t dcpitch, const float *ncurr, size_t ncpitch, const unsigned short *dprev,
+                               size_t dppitch, const float *nprev, size_t nppitch, int cols, int rows, orc_intr k, const orc_aff3f *T,
+                               float dist2_thres, float min_cosine, int x, int y, float row[7])
+{
+    const float finvx = 1.f / k.fx, finvy = 1.f / k.fy;              /* setLevelIntr, projective_icp.cpp:22 */
+    const int src_z = ((const unsigned short *)((const char *)dcurr + (size_t)y * dcpitch))[x];
+    if (src_z == 0) return -1;
+    const float zs = src_z * 0.001f;
+    orc_f3 s = f3(zs * ((float)x - k.cx) * finvx, zs * ((float)y - k.cy) * finvy, zs);
+    s = orc_aff_mul(T, s);
+    float u = fmaf(k.fx, s.x / s.z, k.cx);
+    float v = fmaf(k.fy, s.y / s.z, k.cy);
+    if (s.z <= 0 || u < 0 || v < 0 || u >= (float)cols || v >= (float)rows) return -1;
+    if (!(u == u) || !(v == v)) return -1;
+    const int dst_z = ((const unsigned short *)((const char *)dprev + (size_t)(int)v * dppitch))[(int)u];
+    if (dst_z == 0) return -1;
+    const float zd = dst_z * 0.001f;
+    orc_f3 d = f3(zd * (u - k.cx) * finvx, zd * (v - k.cy) * finvy, zd);
+    orc_f3 df = orc_sub(s, d);
+    float dist2 = orc_dot(df, df);
+    if (dist2 > dist2_thres) return -1;
+    const float *nc = orc_row_f4(ncurr, ncpitch, y) + 4 * x;
+    orc_f3 ns = orc_mat_mul(T->R, f3(nc[0], nc[1], nc[2]));
+    const float *np = orc_row_f4(nprev, nppitch, (int)v) + 4 * (int)u;
+    orc_f3 nd = f3(np[0], np[1], np[2]);
+    float cosine = fabsf(orc_dot(ns, nd));
+    if (!(cosine >= min_cosine)) { if (cosine < min_cosine) return -1; }   /* NaN cosine passes, as in the reference */
+    orc_f3 c = orc_cross(s, nd);
+    row[0] = c.x; row[1] = c.y; row[2] = c.z; row[3] = nd.x; row[4] = nd.y; row[5] = nd.z;
+    row[6] = orc_dot(nd, orc_sub(d, s));
+    return (long long)(int)v * cols + (int)u;
+}
+
+/* the 27 products row_i * row_j (i = 0..5, j = i..6) of one row, formed in float (proj_icp.cu:137-345), added to acc in double */
+static void icp_add_row(double acc[27], const float row[7])
+{
+    int shift = 0;
+    for (int i = 0; i < 6; ++i)
+        for (int j = i; j < 7; ++j) acc[shift++] += (double)(row[i] * row[j]);
+}
+
+/* Per-pixel export of the rule: rows7[7 * (y * cols + x)] receives the pixel's row (NaN x 7 when it is rejected), match[y * cols + x]
+ * the linear index of the matched previous pixel (-1 when rejected).  An accepted row may itself hold NaN (a NaN previous normal passes
+ * the cosine test): match, not the row, tells inliers apart.  Returns the number of inliers. */
+long long orc_icp_rows(const float *vcurr, size_t vcpitch, const float *ncurr, size_t ncpitch, const float *vprev, size_t vppitch,
+                       const float *nprev, size_t nppitch, int cols, int rows, orc_intr k, orc_aff3f T, float dist2_thres, float min_cosine,
+                       float *rows7, int *match)
+{
+    long long inliers = 0;
+    for (int y = 0; y < rows; ++y)
+        for (int x = 0; x < cols; ++x) {
+            float *row = rows7 + 7 * ((size_t)y * cols + x);
+            const long long m = icp_row_points(vcurr, vcpitch, ncurr, ncpitch, vprev, vppitch, nprev, nppitch, cols, rows, k, &T,
+                                               dist2_thres, min_cosine, x, y, row);
+            if (m < 0) for (int i = 0; i < 7; ++i) row[i] = NAN;
+            match[(size_t)y * cols + x] = (int)m;
+            inliers += m >= 0;
+        }
+    return inliers;
+}
+
+long long orc_icp_rows_depth(const unsigned short *dcurr, size_t dcpitch, const float *ncurr, size_t ncpitch, const unsigned short *dprev,
+                             size_t dppitch, const float *nprev, size_t nppitch, int cols, int rows, orc_intr k, orc_aff3f T,
+                             float dist2_thres, float min_cosine, float *rows7, int *match)
+{
+    long long inliers = 0;
+    for (int y = 0; y < rows; ++y)
+        for (int x = 0; x < cols; ++x) {
+            float *row = rows7 + 7 * ((size_t)y * cols + x);
+            const long long m = icp_row_depth(dcurr, dcpitch, ncurr, ncpitch, dprev, dppitch, nprev, nppitch, cols, rows, k, &T,
+                                              dist2_thres, min_cosine, x, y, row);
+            if (m < 0) for (int i = 0; i < 7; ++i) row[i] = NAN;
+            match[(size_t)y * cols + x] = (int)m;
+            inliers += m >= 0;
+        }
+    return inliers;
+}
+
+/* The 27 sums of one level: the rows above summed in raster order, in double (the reference's float tree-sum order is launch-geometry
+ * dependent).  Returns the number of inlier correspondences. */
 long long orc_icp_accumulate(const float *vcurr, size_t vcpitch, const float *ncurr, size_t ncpitch, const float *vprev, size_t vppitch,
                              const float *nprev, size_t nppitch, int cols, int rows, orc_intr k, orc_aff3f T,
                              float dist2_thres, float min_cosine, double *out27)
@@ -19,43 +132,17 @@ long long orc_icp_accumulate(const float *vcurr, size_t vcpitch, const float *nc
     long long inliers = 0;
     for (int y = 0; y < rows; ++y)
         for (int x = 0; x < cols; ++x) {
-            const float *vc = orc_row_f4(vcurr, vcpitch, y) + 4 * x;
-            orc_f3 s = f3(vc[0], vc[1], vc[2]);
-            if (isnan(s.x)) continue;
-            s = orc_aff_mul(&T, s);
-            float u = fmaf(k.fx, s.x / s.z, k.cx);
-            float v = fmaf(k.fy, s.y / s.z, k.cy);
-            if (s.z <= 0 || u < 0 || v < 0 || u >= (float)cols || v >= (float)rows) continue;
-            if (!(u == u) || !(v == v)) continue;
-            const float *dp = orc_row_f4(vprev, vppitch, (int)v) + 4 * (int)u;
-            orc_f3 d = f3(dp[0], dp[1], dp[2]);
-            if (isnan(d.x)) continue;
-            orc_f3 df = orc_sub(s, d);
-            float dist2 = orc_dot(df, df);
-            if (dist2 > dist2_thres) continue;
-            const float *nc = orc_row_f4(ncurr, ncpitch, y) + 4 * x;
-            orc_f3 ns = orc_mat_mul(T.R, f3(nc[0], nc[1], nc[2]));
-            const float *np = orc_row_f4(nprev, nppitch, (int)v) + 4 * (int)u;
-            orc_f3 nd = f3(np[0], np[1], np[2]);
-            float cosine = fabsf(orc_dot(ns, nd));
-            if (!(cosine >= min_cosine)) { if (cosine < min_cosine) continue; }   /* NaN cosine passes, as in the reference */
             float row[7];
-            orc_f3 c = orc_cross(s, nd);
-            row[0] = c.x; row[1] = c.y; row[2] = c.z; row[3] = nd.x; row[4] = nd.y; row[5] = nd.z;
-            row[6] = orc_dot(nd, orc_sub(d, s));
-            int shift = 0;
-            for (int i = 0; i < 6; ++i)
-                for (int j = i; j < 7; ++j) acc[shift++] += (double)(row[i] * row[j]);
+            if (icp_row_points(vcurr, vcpitch, ncurr, ncpitch, vprev, vppitch, nprev, nppitch, cols, rows, k, &T, dist2_thres, min_cosine,
+                               x, y, row) < 0)
+                continue;
+            icp_add_row(acc, row);
             ++inliers;
         }
     for (int i = 0; i < 27; ++i) out27[i] = acc[i];
     return inliers;
 }
 
-/* ComputeIcpHelper::find_coresp, USE_DEPTH variant (proj_icp.cu:47-78; compiled in when internal.hpp:6 defines USE_DEPTH):
- * the source point is the current depth pixel (u16 millimetres) re-projected with finv = 1/f (reproj, proj_icp.cu:39-45), the
- * destination is the previous depth map point-sampled at the projection (texture<ushort> dprev_tex, cudaFilterModePoint) and
- * re-projected at the fractional coordinates; normals as in the points variant.  Row build and sums as above. */
 long long orc_icp_accumulate_depth(const unsigned short *dcurr, size_t dcpitch, const float *ncurr, size_t ncpitch, const unsigned short *dprev,
                                    size_t dppitch, const float *nprev, size_t nppitch, int cols, int rows, orc_intr k, orc_aff3f T,
                                    float dist2_thres, float min_cosine, double *out27)
@@ -63,38 +150,13 @@ long long orc_icp_accumulate_depth(const unsigned short *dcurr, size_t dcpitch, 
     double acc[27];
     for (int i = 0; i < 27; ++i) acc[i] = 0.0;
     long long inliers = 0;
-    const float finvx = 1.f / k.fx, finvy = 1.f / k.fy;              /* setLevelIntr, projective_icp.cpp:22 */
     for (int y = 0; y < rows; ++y)
         for (int x = 0; x < cols; ++x) {
-            const int src_z = ((const unsigned short *)((const char *)dcurr + (size_t)y * dcpitch))[x];
-            if (src_z == 0) continue;
-            const float zs = src_z * 0.001f;
-            orc_f3 s = f3(zs * ((float)x - k.cx) * finvx, zs * ((float)y - k.cy) * finvy, zs);
-            s = orc_aff_mul(&T, s);
-            float u = fmaf(k.fx, s.x / s.z, k.cx);
-            float v = fmaf(k.fy, s.y / s.z, k.cy);
-            if (s.z <= 0 || u < 0 || v < 0 || u >= (float)cols || v >= (float)rows) continue;
-            if (!(u == u) || !(v == v)) continue;
-            const int dst_z = ((const unsigned short *)((const char *)dprev + (size_t)(int)v * dppitch))[(int)u];
-            if (dst_z == 0) continue;
-            const float zd = dst_z * 0.001f;
-            orc_f3 d = f3(zd * (u - k.cx) * finvx, zd * (v - k.cy) * finvy, zd);
-            orc_f3 df = orc_sub(s, d);
-            float dist2 = orc_dot(df, df);
-            if (dist2 > dist2_thres) continue;
-            const float *nc = orc_row_f4(ncurr, ncpitch, y) + 4 * x;
-            orc_f3 ns = orc_mat_mul(T.R, f3(nc[0], nc[1], nc[2]));
-            const float *np = orc_row_f4(nprev, nppitch, (int)v) + 4 * (int)u;
-            orc_f3 nd = f3(np[0], np[1], np[2]);
-            float cosine = fabsf(orc_dot(ns, nd));
-            if (!(cosine >= min_cosine)) { if (cosine < min_cosine) continue; }   /* NaN cosine passes, as in the reference */
             float row[7];
-            orc_f3 c = orc_cross(s, nd);
-            row[0] = c.x; row[1] = c.y; row[2] = c.z; row[3] = nd.x; row[4] = nd.y; row[5] = nd.z;
-            row[6] = orc_dot(nd, orc_sub(d, s));
-            int shift = 0;
-            for (int i = 0; i < 6; ++i)
-                for (int j = i; j < 7; ++j) acc[shift++] += (double)(row[i] * row[j]);
+            if (icp_row_depth(dcurr, dcpitch, ncurr, ncpitch, dprev, dppitch, nprev, nppitch, cols, rows, k, &T, dist2_thres, min_cosine,
+                              x, y, row) < 0)
+                continue;
+            icp_add_row(acc, row);
             ++inliers;
         }
     for (int i = 0; i < 27; ++i) out27[i] = acc[i];
