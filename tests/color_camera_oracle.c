@@ -5,49 +5,13 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "oracle_util.h"
+
 /* the rule's constants, restated here rather than taken from dfusion.h so that a change there shows as a disagreement */
 #define COLOR_BAND 0.5f
 #define COLOR_OCCLUSION 1.0f
 #define ACTIVITY_VOXELS 1024
 #define MAP_EMPTY 0xffffffffu
-
-static float half_to_float(uint16_t h)
-{
-    const uint32_t sign = (uint32_t)(h & 0x8000u) << 16, exp = (h >> 10) & 0x1fu, man = h & 0x3ffu;
-    uint32_t bits;
-    if (exp == 0) {
-        if (man == 0) bits = sign;
-        else {
-            const float f = (float)man * (1.0f / 16777216.0f);
-            memcpy(&bits, &f, 4);
-            bits |= sign;
-        }
-    } else if (exp == 31) bits = sign | 0x7f800000u | (man << 13);
-    else bits = sign | ((exp + 112u) << 23) | (man << 13);
-    float out;
-    memcpy(&out, &bits, 4);
-    return out;
-}
-
-static uint32_t float_bits(float f)
-{
-    uint32_t u;
-    memcpy(&u, &f, 4);
-    return u;
-}
-
-static float bits_float(uint32_t u)
-{
-    float f;
-    memcpy(&f, &u, 4);
-    return f;
-}
-
-/* a12: R row-major then t; out = R p + t as fma(r.x, p.x, fma(r.y, p.y, r.z * p.z)) + t */
-static void aff_apply(const float *a12, const float *p, float *out)
-{
-    for (int c = 0; c < 3; ++c) out[c] = fmaf(a12[3 * c], p[0], fmaf(a12[3 * c + 1], p[1], a12[3 * c + 2] * p[2])) + a12[9 + c];
-}
 
 /* cam4: colour fx, fy, cx, cy; returns 1 and the colour pixel (u, v) when pc lies in front of the colour camera and inside its image */
 static int project_color(const float *pc, const float *cam4, int ccols, int crows, float *u, float *v)

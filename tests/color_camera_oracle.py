@@ -1,40 +1,23 @@
-"""ctypes binding of the colour-camera oracle (tests/color_camera_oracle.c), test infrastructure only.  The C file is compiled on first use
-into a fresh temporary directory, so a read-only checkout works too."""
+"""ctypes binding of the colour-camera oracle (tests/color_camera_oracle.c), test infrastructure only."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
+import c_oracle
 import color_oracle as co
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "color_camera_oracle.c"
 EMPTY = 0xFFFFFFFF
-_lib = None
 
 
 def load() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        cc = "/usr/bin/gcc" if Path("/usr/bin/gcc").exists() else (shutil.which("gcc") or "cc")
-        out = Path(tempfile.mkdtemp(prefix="color_camera_oracle_")) / "libcolor_camera_oracle.so"
-        subprocess.run([cc, "-std=gnu11", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-shared", "-o", str(out),
-                        str(SRC), "-lm"], check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-        lib = C.CDLL(str(out))
-        vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
-        lib.cc_cell.restype = i
-        lib.cc_cell.argtypes = [vp, vp]
-        lib.cc_depth_map.restype = None
-        lib.cc_depth_map.argtypes = [vp, sz, i, i, vp, i, i, vp, vp, vp, sz]
-        lib.cc_integrate_color_camera.restype = None
-        lib.cc_integrate_color_camera.argtypes = [vp, vp, f, i, vp, vp, sz, i, i, vp, vp, i, i, vp, vp, vp, sz, vp, sz, vp]
-        _lib = lib
-    return _lib
+    vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    return c_oracle.load("color_camera_oracle", {
+        "cc_cell": (i, [vp, vp]),
+        "cc_depth_map": (None, [vp, sz, i, i, vp, i, i, vp, vp, vp, sz]),
+        "cc_integrate_color_camera": (None, [vp, vp, f, i, vp, vp, sz, i, i, vp, vp, i, i, vp, vp, vp, sz, vp, sz, vp]),
+    })
 
 
 class Camera:

@@ -6,28 +6,11 @@
 #include <string.h>
 
 #include "df_hostmath.h"
+#include "oracle_util.h"
 
 /* the rule's constants, restated here rather than taken from dfusion.h so that a change there shows as a disagreement */
 #define COLOR_BAND 0.5f
 #define ACTIVITY_VOXELS 1024
-
-static float half_to_float(uint16_t h)
-{
-    const uint32_t sign = (uint32_t)(h & 0x8000u) << 16, exp = (h >> 10) & 0x1fu, man = h & 0x3ffu;
-    uint32_t bits;
-    if (exp == 0) {
-        if (man == 0) bits = sign;
-        else {                                              /* subnormal: man * 2^-24, exact in float */
-            const float f = (float)man * (1.0f / 16777216.0f);
-            memcpy(&bits, &f, 4);
-            bits |= sign;
-        }
-    } else if (exp == 31) bits = sign | 0x7f800000u | (man << 13);
-    else bits = sign | ((exp + 112u) << 23) | (man << 13);
-    float out;
-    memcpy(&out, &bits, 4);
-    return out;
-}
 
 /* dims, vs, trunc_dist, max_weight: the df_volume's; colors: Dx*Dy*Dz words, updated in place; activity may be NULL; pitches in bytes */
 void cl_integrate_color(const int *dims, const float *vs, float trunc_dist, int max_weight, uint32_t *colors, const uint16_t *dists,
@@ -103,8 +86,6 @@ void cl_sample_colors(const int *dims, const float *vs, const uint32_t *colors, 
         rgba[q] = round_channel(s[0] / sw) | (round_channel(s[1] / sw) << 8) | (round_channel(s[2] / sw) << 16) | 0xff000000u;
     }
 }
-
-static float dot(const float *a, const float *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
 /* tri_ids (npix), points (npix * 4): a df_raster_mesh result for verts / tris / w12; vert_rgba: n_verts words; image: npix * 4 bytes B, G, R, 0.
  * weights (optional, npix * 3): b0, b1, b2 per pixel, NaN where there are none */

@@ -1,42 +1,22 @@
-"""ctypes binding of the colour oracle (tests/color_oracle.c), test infrastructure only.  The C file is compiled on first use into a fresh
-temporary directory, so a read-only checkout works too."""
+"""ctypes binding of the colour oracle (tests/color_oracle.c), test infrastructure only."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "color_oracle.c"
-_lib = None
+import c_oracle
 
 
 def load() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        cc = "/usr/bin/gcc" if Path("/usr/bin/gcc").exists() else (shutil.which("gcc") or "cc")
-        out = Path(tempfile.mkdtemp(prefix="color_oracle_")) / "libcolor_oracle.so"
-        subprocess.run([cc, "-std=gnu11", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-shared",
-                        "-I", str(HERE.parent / "include"), "-o", str(out), str(SRC), "-lm"], check=True, stdout=subprocess.PIPE,
-                       stderr=subprocess.STDOUT)
-        lib = C.CDLL(str(out))
-        vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
-        lib.cl_integrate_color.restype = None
-        lib.cl_integrate_color.argtypes = [vp, vp, f, i, vp, vp, sz, vp, sz, i, i, vp, vp, vp]
-        lib.cl_sample_colors.restype = None
-        lib.cl_sample_colors.argtypes = [vp, vp, vp, vp, f, vp, i, sz, vp]
-        lib.cl_mesh_colors.restype = None
-        lib.cl_mesh_colors.argtypes = [vp, vp, vp, i, i, vp, i, vp, vp, sz, vp, vp]
-        lib.cl_aff_mul.restype = None
-        lib.cl_aff_mul.argtypes = [vp, vp, vp]
-        lib.cl_aff_inv.restype = None
-        lib.cl_aff_inv.argtypes = [vp, vp]
-        _lib = lib
-    return _lib
+    vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    return c_oracle.load("color_oracle", {
+        "cl_integrate_color": (None, [vp, vp, f, i, vp, vp, sz, vp, sz, i, i, vp, vp, vp]),
+        "cl_sample_colors": (None, [vp, vp, vp, vp, f, vp, i, sz, vp]),
+        "cl_mesh_colors": (None, [vp, vp, vp, i, i, vp, i, vp, vp, sz, vp, vp]),
+        "cl_aff_mul": (None, [vp, vp, vp]),
+        "cl_aff_inv": (None, [vp, vp]),
+    })
 
 
 def a12(aff):

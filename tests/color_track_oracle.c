@@ -6,13 +6,9 @@
 #include <stdint.h>
 #include <string.h>
 
-static float luma(uint32_t r, uint32_t g, uint32_t b) { return (float)((77u * r + 150u * g + 29u * b + 128u) >> 8) / 255.f; }
+#include "oracle_util.h"
 
-/* the rows of an affine (R row-major, t) applied as the device's aff_mul: fma(r.x, p.x, fma(r.y, p.y, r.z * p.z)) + t */
-static void aff_apply(const float *a12, const float *p, float *out)
-{
-    for (int c = 0; c < 3; ++c) out[c] = fmaf(a12[3 * c], p[0], fmaf(a12[3 * c + 1], p[1], a12[3 * c + 2] * p[2])) + a12[9 + c];
-}
+static float luma(uint32_t r, uint32_t g, uint32_t b) { return (float)((77u * r + 150u * g + 29u * b + 128u) >> 8) / 255.f; }
 
 /* level 0, registered image: out[y * cols + x] = intensity of bgra pixel (x, y) */
 void ct_intensity_registered(const uint8_t *bgra, size_t pitch, int cols, int rows, float *out)

@@ -1,44 +1,25 @@
-"""ctypes binding of the colour-tracking oracle (tests/color_track_oracle.c), test infrastructure only.  The C file is compiled on first use
-into a fresh temporary directory, so a read-only checkout works too."""
+"""ctypes binding of the colour-tracking oracle (tests/color_track_oracle.c), test infrastructure only."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
+import c_oracle
 import color_oracle as co
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "color_track_oracle.c"
 OCCLUSION = 1.0                                             # DF_COLOR_OCCLUSION
-_lib = None
 
 
 def load() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        cc = "/usr/bin/gcc" if Path("/usr/bin/gcc").exists() else (shutil.which("gcc") or "cc")
-        out = Path(tempfile.mkdtemp(prefix="color_track_oracle_")) / "libcolor_track_oracle.so"
-        subprocess.run([cc, "-std=gnu11", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-shared", "-o", str(out),
-                        str(SRC), "-lm"], check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-        lib = C.CDLL(str(out))
-        vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
-        lib.ct_intensity_registered.restype = None
-        lib.ct_intensity_registered.argtypes = [vp, sz, i, i, vp]
-        lib.ct_intensity_camera.restype = None
-        lib.ct_intensity_camera.argtypes = [vp, sz, i, i, vp, vp, i, vp, sz, f, f, vp, i, i, vp]
-        lib.ct_intensity_down.restype = None
-        lib.ct_intensity_down.argtypes = [vp, i, vp, i, i]
-        lib.ct_model_intensity.restype = None
-        lib.ct_model_intensity.argtypes = [vp, vp, vp, vp, vp, i, i, vp, vp]
-        lib.ct_photo_rows.restype = C.c_long
-        lib.ct_photo_rows.argtypes = [vp, vp, vp, vp, i, i, vp, vp, f, f, vp]
-        _lib = lib
-    return _lib
+    vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    return c_oracle.load("color_track_oracle", {
+        "ct_intensity_registered": (None, [vp, sz, i, i, vp]),
+        "ct_intensity_camera": (None, [vp, sz, i, i, vp, vp, i, vp, sz, f, f, vp, i, i, vp]),
+        "ct_intensity_down": (None, [vp, i, vp, i, i]),
+        "ct_model_intensity": (None, [vp, vp, vp, vp, vp, i, i, vp, vp]),
+        "ct_photo_rows": (C.c_long, [vp, vp, vp, vp, i, i, vp, vp, f, f, vp]),
+    })
 
 
 def luma(r, g, b):

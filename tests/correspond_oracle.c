@@ -1,14 +1,11 @@
 /* correspond_oracle.c -- plain C statement of df_mesh_correspond's rule (include/dfusion.h): per pixel of a df_raster_mesh view, the point at
  * the same barycentric position on the source vertex set and the source triangle's face normal; test infrastructure only.  Compiled with
- * -ffp-contract=off so that every float operation is the one the rule names.  Also exposes df_hostmath.h's affine product and inverse, so
- * that tests form the cameras of the frame loop with its own bits. */
+ * -ffp-contract=off so that every float operation is the one the rule names. */
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
 
-#include "df_hostmath.h"
-
-static float dot(const float *a, const float *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+#include "oracle_util.h"
 
 /* tri_ids (cols*rows), points (cols*rows*4): a df_raster_mesh result for verts / tris / w12 (world-to-camera, 12 floats); src: the source
  * vertex set (n_verts x vstride); target (cols*rows*4) may be NULL; out_pts, out_nrm: cols*rows*4 floats */
@@ -91,6 +88,3 @@ void co_weights(const int32_t *tri_ids, const float *points, const float *verts,
         o[0] = 1.f - o[1] - o[2];
     }
 }
-
-void co_aff_mul(const float *a, const float *b, float *out) { dfh_aff_mul(a, b, out); }
-void co_aff_inv(const float *a, float *out) { dfh_aff_inv(a, out); }

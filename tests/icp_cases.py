@@ -124,6 +124,11 @@ POSES = {
 }
 
 
+def acc_id(case):
+    """the test id of an accumulate case (size, variant, pose)"""
+    return f"{case[0][0]}x{case[0][1]}-{case[1]}-{case[2]}"
+
+
 def accumulate_case(cols, rows, variant, pose):
     """(curr maps, prev maps, K, T, dist2, min_cos): the umbrella at this size; maps are (vertex | depth, normal)"""
     Kl = synth.scaled_K(cols, rows)

@@ -1,8 +1,8 @@
 /* lens_oracle.c -- plain C statement of the lens rules of include/dfusion.h: the distortion of df_lens, df_undistort, and the colour
  * camera's projection through its lens in df_color_depth_map_lens, df_integrate_color_camera_lens and df_frame_intensity_lens; test
- * infrastructure only.  It includes color_camera_oracle.c for the colour-camera rules' shared pieces (the affine, fp16, the cell rule, the
- * pinhole projection a NULL lens takes).  Compiled with -ffp-contract=off so that every float operation is the one the rule names; fmaf()
- * only where the rule writes fma. */
+ * infrastructure only.  It includes color_camera_oracle.c for the colour-camera rules' shared pieces (the cell rule, the pinhole projection a
+ * NULL lens takes, and through it oracle_util.h's affine and fp16 helpers).  Compiled with -ffp-contract=off so that every float operation
+ * is the one the rule names; fmaf() only where the rule writes fma. */
 #include "color_camera_oracle.c"
 
 /* lens: k1, k2, p1, p2, k3, k4, k5, k6, r2_max (df_lens' field order); returns 0 when (x, y) is outside the calibrated radius or NaN */

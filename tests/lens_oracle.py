@@ -1,44 +1,24 @@
-"""ctypes binding of the lens oracle (tests/lens_oracle.c), test infrastructure only.  The C file is compiled on first use into a fresh
-temporary directory, so a read-only checkout works too."""
+"""ctypes binding of the lens oracle (tests/lens_oracle.c), test infrastructure only."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
+import c_oracle
 import color_oracle as co
 import color_camera_oracle as cco
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "lens_oracle.c"
-_lib = None
-
 
 def load() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        cc = "/usr/bin/gcc" if Path("/usr/bin/gcc").exists() else (shutil.which("gcc") or "cc")
-        out = Path(tempfile.mkdtemp(prefix="lens_oracle_")) / "liblens_oracle.so"
-        subprocess.run([cc, "-std=gnu11", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-shared", "-I", str(HERE),
-                        "-o", str(out), str(SRC), "-lm"], check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-        lib = C.CDLL(str(out))
-        vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
-        lib.lens_distort.restype = i
-        lib.lens_distort.argtypes = [vp, f, f, C.POINTER(f), C.POINTER(f)]
-        lib.lens_undistort.restype = None
-        lib.lens_undistort.argtypes = [vp, sz, vp, sz, vp, sz, vp, sz, i, i, vp, vp]
-        lib.lens_depth_map.restype = None
-        lib.lens_depth_map.argtypes = [vp, sz, i, i, vp, i, i, vp, vp, vp, vp, sz]
-        lib.lens_integrate_color_camera.restype = None
-        lib.lens_integrate_color_camera.argtypes = [vp, vp, f, i, vp, vp, sz, i, i, vp, vp, i, i, vp, vp, vp, vp, sz, vp, sz, vp]
-        lib.lens_frame_intensity.restype = None
-        lib.lens_frame_intensity.argtypes = [vp, sz, i, i, vp, vp, vp, vp, vp, sz, f, vp, i, i, vp]
-        _lib = lib
-    return _lib
+    vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    return c_oracle.load("lens_oracle", {
+        "lens_distort": (i, [vp, f, f, C.POINTER(f), C.POINTER(f)]),
+        "lens_undistort": (None, [vp, sz, vp, sz, vp, sz, vp, sz, i, i, vp, vp]),
+        "lens_depth_map": (None, [vp, sz, i, i, vp, i, i, vp, vp, vp, vp, sz]),
+        "lens_integrate_color_camera": (None, [vp, vp, f, i, vp, vp, sz, i, i, vp, vp, i, i, vp, vp, vp, vp, sz, vp, sz, vp]),
+        "lens_frame_intensity": (None, [vp, sz, i, i, vp, vp, vp, vp, vp, sz, f, vp, i, i, vp]),
+    })
 
 
 def lens9(lens):

@@ -1,11 +1,12 @@
 /* mesh_oracle.c -- CPU restatement of the mesh extraction (dfusion.h df_mesh_*, csrc/mesh.cu) for the tests: a plain loop over the cubes in
  * the documented order.  Vertex indices come from a dense per-(voxel, axis) map of the cloud, numbered in the order the cloud extraction
  * emits its points (ascending (z, y, x), then +x, +y, +z) and under its conditions (orc_extract_cloud, oracle/orc_tsdf.c; the tests check
- * the map against that function's output point by point).  Self-contained: built and loaded by tests/mesh_oracle.py. */
+ * the map against that function's output point by point).  Built and loaded by tests/mesh_oracle.py. */
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
-#include "../include/df_mc_table.h"
+#include "df_mc_table.h"
+#include "oracle_util.h"
 
 static const signed char TRIS[256][DF_MC_ROW] = DF_MC_TRIANGLES_INIT;
 static const signed char CORNER[8][3] = DF_MC_CORNER_INIT;
@@ -13,21 +14,10 @@ static const signed char OWNER[12][4] = DF_MC_EDGE_OWNER_INIT;
 
 typedef struct { uint32_t *data; int dims[3]; } mo_volume;
 
-/* IEEE half -> float, exact */
-static float half2float(uint16_t h)
-{
-    const int e = (h >> 10) & 0x1f, m = h & 0x3ff;
-    float f;
-    if (e == 0) f = ldexpf((float)m, -24);
-    else if (e == 31) f = m ? NAN : INFINITY;
-    else f = ldexpf((float)(m | 0x400), e - 25);
-    return (h & 0x8000) ? -f : f;
-}
-
 /* a voxel takes part in extraction iff W != 0 && F != 1 */
 static int active(uint32_t v, float *F)
 {
-    *F = half2float((uint16_t)(v & 0xffffu));
+    *F = half_to_float((uint16_t)(v & 0xffffu));
     return (v >> 16) != 0 && *F != 1.f;
 }
 

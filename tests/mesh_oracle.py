@@ -1,18 +1,11 @@
-"""ctypes binding of the mesh oracle (tests/mesh_oracle.c), test infrastructure only.  The C file is compiled on first use into a fresh
-temporary directory, so a read-only checkout works too."""
+"""ctypes binding of the mesh oracle (tests/mesh_oracle.c), test infrastructure only."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "mesh_oracle.c"
-_lib = None
+import c_oracle
 
 
 class _Volume(C.Structure):
@@ -20,19 +13,10 @@ class _Volume(C.Structure):
 
 
 def load() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        cc = "/usr/bin/gcc" if Path("/usr/bin/gcc").exists() else (shutil.which("gcc") or "cc")
-        out = Path(tempfile.mkdtemp(prefix="mesh_oracle_")) / "libmesh_oracle.so"
-        subprocess.run([cc, "-std=gnu11", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-shared", "-o", str(out),
-                        str(SRC), "-lm"], check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-        lib = C.CDLL(str(out))
-        lib.mo_vertex_map.restype = C.c_longlong
-        lib.mo_vertex_map.argtypes = [_Volume, C.c_void_p]
-        lib.mo_mesh.restype = C.c_longlong
-        lib.mo_mesh.argtypes = [_Volume, C.c_longlong, C.c_void_p, C.c_longlong]
-        _lib = lib
-    return _lib
+    return c_oracle.load("mesh_oracle", {
+        "mo_vertex_map": (C.c_longlong, [_Volume, C.c_void_p]),
+        "mo_mesh": (C.c_longlong, [_Volume, C.c_longlong, C.c_void_p, C.c_longlong]),
+    })
 
 
 def _vol(vol_data: np.ndarray, dims) -> _Volume:

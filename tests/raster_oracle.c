@@ -8,7 +8,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include "df_hostmath.h"
+#include "oracle_util.h"
 
 #define NEAR 0.01f
 #define GUARD 16777216.f
@@ -30,7 +30,6 @@ static void cross(const float *a, const float *b, float *o)
     o[1] = a[2] * b[0] - a[0] * b[2];
     o[2] = a[0] * b[1] - a[1] * b[0];
 }
-static float dot(const float *a, const float *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 static int imin(int a, int b) { return a < b ? a : b; }
 static int imax(int a, int b) { return a > b ? a : b; }
 
@@ -98,8 +97,6 @@ static void ray(const intr *K, float finvx, float finvy, int i, int j, float *d)
     d[2] = 1.f;
 }
 
-static uint32_t fbits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
-
 /* the renderer: tri_ids (cols*rows, may be NULL), points and normals (cols*rows*4 floats), stats (5, may be NULL); returns 0, or -1 when
  * out of memory */
 int ro_raster(const float *verts, int n_verts, int vstride, const int32_t *tris, int n_tris, const float *w12, const float *k4, int cols,
@@ -128,7 +125,7 @@ int ro_raster(const float *verts, int n_verts, int vstride, const int32_t *tris,
                 ray(&K, finvx, finvy, i, j, d);
                 const float tz = T.num / dot(T.n, d);
                 if (!(tz > 0.f && tz < INFINITY)) continue;
-                const unsigned long long key = ((unsigned long long)fbits(tz) << 32) | (uint32_t)t;
+                const unsigned long long key = ((unsigned long long)float_bits(tz) << 32) | (uint32_t)t;
                 if (key < z[(size_t)j * cols + i]) z[(size_t)j * cols + i] = key;
             }
     }
@@ -162,9 +159,6 @@ int ro_raster(const float *verts, int n_verts, int vstride, const int32_t *tris,
     free(cam); free(fix); free(z);
     return 0;
 }
-
-/* the inverse df_kinfu_render applies to a camera-to-model pose (12 floats, R row-major then t) */
-void ro_aff_inv(const float *aff, float *out) { dfh_aff_inv(aff, out); }
 
 /* per pixel, the number of drawn (front-facing, not skipped) triangles whose sample test covers it; no depth test */
 int ro_coverage(const float *verts, int n_verts, int vstride, const int32_t *tris, int n_tris, const float *w12, const float *k4, int cols,

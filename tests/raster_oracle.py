@@ -1,48 +1,28 @@
-"""ctypes binding of the rasteriser oracle (tests/raster_oracle.c), test infrastructure only.  The C file is compiled on first use into a
-fresh temporary directory, so a read-only checkout works too."""
+"""ctypes binding of the rasteriser oracle (tests/raster_oracle.c), test infrastructure only."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
-HERE = Path(__file__).resolve().parent
-SRC = HERE / "raster_oracle.c"
-_lib = None
+import c_oracle
+import color_oracle as co
 
 
 def load() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        cc = "/usr/bin/gcc" if Path("/usr/bin/gcc").exists() else (shutil.which("gcc") or "cc")
-        out = Path(tempfile.mkdtemp(prefix="raster_oracle_")) / "libraster_oracle.so"
-        subprocess.run([cc, "-std=gnu11", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-shared",
-                        "-I", str(HERE.parent / "include"), "-o", str(out), str(SRC), "-lm"], check=True, stdout=subprocess.PIPE,
-                       stderr=subprocess.STDOUT)
-        lib = C.CDLL(str(out))
-        lib.ro_aff_inv.restype = None
-        lib.ro_aff_inv.argtypes = [C.c_void_p, C.c_void_p]
-        args = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-        lib.ro_raster.restype = C.c_int
-        lib.ro_raster.argtypes = args + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.ro_coverage.restype = C.c_int
-        lib.ro_coverage.argtypes = args + [C.c_void_p]
-        _lib = lib
-    return _lib
+    args = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    return c_oracle.load("raster_oracle", {
+        "ro_raster": (C.c_int, args + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+        "ro_coverage": (C.c_int, args + [C.c_void_p]),
+    })
 
 
 def _inputs(verts, tris, world2cam, K):
     v = np.ascontiguousarray(verts, np.float32)
     assert v.ndim == 2 and v.shape[1] in (3, 4)
     t = np.ascontiguousarray(np.asarray(tris, np.int32).reshape(-1, 3))
-    R, tr = world2cam
-    w = np.concatenate([np.asarray(R, np.float32).reshape(9), np.asarray(tr, np.float32).reshape(3)]).astype(np.float32)
     k = np.asarray(K, np.float32).reshape(4)
-    return v, t, w, k
+    return v, t, co.a12(world2cam), k
 
 
 def raster(verts, tris, world2cam, K, cols, rows):
@@ -57,14 +37,6 @@ def raster(verts, tris, world2cam, K, cols, rows):
                          pts.ctypes.data, nrm.ctypes.data, stats.ctypes.data)
     assert r == 0
     return ids, pts, nrm, stats
-
-
-def aff_inv(R, t):
-    """(R, t)^-1 as df_kinfu_render computes it (df_hostmath.h dfh_aff_inv), float32"""
-    a = np.concatenate([np.asarray(R, np.float32).reshape(9), np.asarray(t, np.float32).reshape(3)]).astype(np.float32)
-    out = np.empty(12, np.float32)
-    load().ro_aff_inv(a.ctypes.data, out.ctypes.data)
-    return out[:9].reshape(3, 3), out[9:]
 
 
 def coverage(verts, tris, world2cam, K, cols, rows):

@@ -1,6 +1,5 @@
 """CPU checks of the colour feature: the three rules of include/dfusion.h as tests/color_oracle.c states them (closed forms on small scenes),
 the synthetic RGB-D scene, the coloured PLY export and the version-2 snapshot checks of df_kinfu_snapshot_params (host code)."""
-import ctypes as C
 import struct
 
 import numpy as np
@@ -8,28 +7,8 @@ import pytest
 
 import color_oracle as co
 import snapshot_model as sm
-
-DIMS = (32, 24, 20)
-VS = (0.02, 0.02, 0.02)
-TRUNC = 0.06
-BAND = 0.5 * TRUNC
-COLS, ROWS = 64, 48
-K = (60.0, 60.0, 32.0, 24.0)
-VOL2CAM = (np.eye(3, dtype=np.float32), np.array([-0.32, -0.24, 0.5], np.float32))
-PLANE_Z = 0.7
-
-
-def plane_dists(z=PLANE_Z):
-    u, v = np.meshgrid(np.arange(COLS, dtype=np.float64), np.arange(ROWS, dtype=np.float64))
-    ray = np.sqrt(((u - K[2]) / K[0]) ** 2 + ((v - K[3]) / K[1]) ** 2 + 1.0)
-    return (z * ray).astype(np.float16).view(np.uint16)
-
-
-def constant_image(bgr):
-    img = np.empty((ROWS, COLS, 4), np.uint8)
-    img[..., :3] = bgr
-    img[..., 3] = 255
-    return img
+from scenes import BAND, COLS, DIMS, K, ROWS, TRUNC, VOL2CAM, VS, constant_image, plane_dists, word
+from snapshot_model import lib  # noqa: F401  (a fixture)
 
 
 def voxel_sdf(dists):
@@ -46,10 +25,6 @@ def voxel_sdf(dists):
 
 def integrate(colors, img, dists=None, activity=None, max_weight=64):
     return co.integrate_color(colors, DIMS, VS, TRUNC, max_weight, plane_dists() if dists is None else dists, img, VOL2CAM, K, activity)
-
-
-def word(r, g, b, w):
-    return r | (g << 8) | (b << 16) | (w << 24)
 
 
 def test_plane_colours_exactly_the_band():
@@ -239,83 +214,36 @@ def test_save_ply_with_colours(tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------------------------------- snapshots
-@pytest.fixture(scope="module")
-def lib():
-    from dynamicfusion_b200 import build, capi
-    build.build()
-    return capi.load()
-
-
-def _params(capi, lib, flags):
-    p = capi.KinfuParams()
-    lib.df_kinfu_default_params(C.byref(p), 0)
-    p.cols, p.rows = 64, 48
-    for i in range(3):
-        p.volume_dims[i] = (32, 24, 20)[i]
-    p.icp_iter_num[:] = [3, 2, 0, 0]
-    p.cloud_capacity = 1000
-    p.flags = flags
-    return p
-
-
-def _v1_body(capi, lib, p, cloud=5):
-    dims = tuple(p.volume_dims)
-    vol = capi.make_volume(None, dims, (1.0, 1.0, 1.0), 0.1, 64)
-    pyr = sum((p.cols >> l) * (p.rows >> l) * 32 for l in range(2))
-    rng = np.random.default_rng(3)
-    body = bytes(p) + bytes(capi.F2Params()) + sm.COUNTERS.pack(4, 1, 1, 3, cloud, 2, 0, 4 * 7)
-    body += rng.random(2 * 12, np.float32).tobytes() + rng.random(3 * 12, np.float32).tobytes()
-    body += bytes(lib.df_volume_activity_bytes(vol)) + rng.random(pyr // 4, np.float32).tobytes() + rng.random(cloud * 8, np.float32).tobytes()
-    body += bytes(sm.brick_count(dims)) + rng.integers(0, 2 ** 32, 7, np.uint32).tobytes()
-    return body
-
-
-def _color_sections(dims, cloud=5):
-    """version 2's trailing sections for a colour volume with one uniform and one mixed brick"""
-    vol = np.zeros(dims[::-1], np.uint32)
-    vol[0:8, 0:8, 0:8] = word(1, 2, 3, 4)
-    vol[8:16, 8:12, 0:5] = word(9, 9, 9, 1)
-    cls, payload = sm.pack(vol.reshape(-1), dims)
-    assert sorted(np.unique(cls)) == [0, 1, 2] and len(payload) == 1 + 512
-    return struct.pack("<Q", 4 * len(payload)), cls.tobytes(), payload.tobytes(), np.arange(cloud, dtype=np.uint32).tobytes()
-
-
-def _call(lib, capi, data: bytes):
-    out = capi.KinfuParams()
-    buf = np.frombuffer(data, np.uint8)
-    return lib.df_kinfu_snapshot_params(buf.ctypes.data, len(data), C.byref(out)), out
-
-
 def test_snapshot_version_2_checks(lib):
     from dynamicfusion_b200 import capi
     from dynamicfusion_b200.kinfu import COLOR
-    p1, p2 = _params(capi, lib, 0), _params(capi, lib, COLOR)
+    p1, p2 = sm.small_params(capi, lib, 0), sm.small_params(capi, lib, COLOR)
     dims = tuple(p2.volume_dims)
-    v1 = _v1_body(capi, lib, p1)
-    st, out = _call(lib, capi, sm.header(v1) + v1)
+    v1 = sm.v1_body(capi, lib, p1)
+    st, out = sm.read_params(lib, capi, sm.header(v1) + v1)
     assert st == 0 and bytes(out) == bytes(p1)                          # a version-1 byte string is still accepted
-    length, cls, payload, rgba = _color_sections(dims)
-    body = _v1_body(capi, lib, p2) + length + cls + payload + rgba
+    length, cls, payload, rgba = sm.color_sections(dims)
+    body = sm.v1_body(capi, lib, p2) + length + cls + payload + rgba
     snap = sm.header(body, version=2) + body
-    st, out = _call(lib, capi, snap)
+    st, out = sm.read_params(lib, capi, snap)
     assert st == 0 and bytes(out) == bytes(p2) and out.flags & COLOR
 
     def rejected(b, version=2):
-        return _call(lib, capi, sm.header(b, version=version) + b)[0] != 0
+        return sm.read_params(lib, capi, sm.header(b, version=version) + b)[0] != 0
     assert rejected(body, version=1)                                    # the version must match the colour flag
     assert rejected(v1, version=2)
     assert rejected(body, version=3)
     assert rejected(body[:-4])                                          # a colour word short
     assert rejected(body + b"\0\0\0\0")
-    assert rejected(_v1_body(capi, lib, p2))                            # the colour sections missing altogether
+    assert rejected(sm.v1_body(capi, lib, p2))                          # the colour sections missing altogether
     bad = bytearray(cls); bad[5] = 3
-    assert rejected(_v1_body(capi, lib, p2) + length + bytes(bad) + payload + rgba)
+    assert rejected(sm.v1_body(capi, lib, p2) + length + bytes(bad) + payload + rgba)
     swap = bytearray(cls); swap[list(cls).index(1)] = 2                 # classes that imply another payload length
-    assert rejected(_v1_body(capi, lib, p2) + length + bytes(swap) + payload + rgba)
-    assert rejected(_v1_body(capi, lib, p2) + struct.pack("<Q", 4 * 512) + cls + payload[4:] + rgba)
-    assert rejected(_v1_body(capi, lib, p2) + struct.pack("<Q", 2 ** 62) + cls + payload + rgba)
+    assert rejected(sm.v1_body(capi, lib, p2) + length + bytes(swap) + payload + rgba)
+    assert rejected(sm.v1_body(capi, lib, p2) + struct.pack("<Q", 4 * 512) + cls + payload[4:] + rgba)
+    assert rejected(sm.v1_body(capi, lib, p2) + struct.pack("<Q", 2 ** 62) + cls + payload + rgba)
     corrupt = bytearray(snap); corrupt[-10] ^= 1                        # the checksum covers the colour sections
-    assert _call(lib, capi, bytes(corrupt))[0] != 0
+    assert sm.read_params(lib, capi, bytes(corrupt))[0] != 0
 
 
 def test_cpp_colour_export_builds():

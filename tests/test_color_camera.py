@@ -10,8 +10,8 @@ import pytest
 import color_camera_oracle as cco
 import color_oracle as co
 import snapshot_model as sm
-from test_color import (BAND, COLS, DIMS, K, ROWS, TRUNC, VOL2CAM, VS, _call, _color_sections, _params, _v1_body, constant_image,
-                        lib, plane_dists, word)  # noqa: F401  (lib is a fixture)
+from scenes import COLS, DIMS, K, ROWS, TRUNC, VOL2CAM, VS, constant_image, plane_dists
+from snapshot_model import lib  # noqa: F401  (a fixture)
 
 IDENTITY = (np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
 
@@ -189,12 +189,6 @@ def test_colour_pixel_comes_from_the_colour_camera():
 
 
 # ------------------------------------------------------------------------------------------------------------------------- snapshots
-def _camera_bytes(capi, K_=(1081.0, 1081.0, 959.5, 539.5), cols=1920, rows=1080, t=(0.052, 0.0, 0.0)):
-    cam = capi.make_color_camera(K_, cols, rows, ((1, 0, 0, 0, 1, 0, 0, 0, 1), t))
-    assert C.sizeof(cam) == 72
-    return bytes(cam)
-
-
 def _snapshot_camera(lib, capi, data):
     cam, present = capi.ColorCamera(), C.c_int(-1)
     buf = np.frombuffer(data, np.uint8)
@@ -205,32 +199,32 @@ def _snapshot_camera(lib, capi, data):
 def test_snapshot_version_3_checks(lib):
     from dynamicfusion_b200 import capi
     from dynamicfusion_b200.kinfu import COLOR
-    p1, p2 = _params(capi, lib, 0), _params(capi, lib, COLOR)
+    p1, p2 = sm.small_params(capi, lib, 0), sm.small_params(capi, lib, COLOR)
     dims = tuple(p2.volume_dims)
-    length, cls, payload, rgba = _color_sections(dims)
-    v2 = _v1_body(capi, lib, p2) + length + cls + payload + rgba
-    cam = _camera_bytes(capi)
+    length, cls, payload, rgba = sm.color_sections(dims)
+    v2 = sm.v1_body(capi, lib, p2) + length + cls + payload + rgba
+    cam = sm.camera_bytes(capi)
     v3 = v2 + cam
     snap = sm.header(v3, version=3) + v3
-    st, out = _call(lib, capi, snap)
+    st, out = sm.read_params(lib, capi, snap)
     assert st == 0 and bytes(out) == bytes(p2)
     assert _snapshot_camera(lib, capi, snap) == (0, 1, cam)
     assert _snapshot_camera(lib, capi, sm.header(v2, version=2) + v2) == (0, 0, bytes(72))   # version 2: no camera
-    v1 = _v1_body(capi, lib, p1)
+    v1 = sm.v1_body(capi, lib, p1)
     assert _snapshot_camera(lib, capi, sm.header(v1) + v1) == (0, 0, bytes(72))
 
     def rejected(b, version=3):
         data = sm.header(b, version=version) + b
-        return _call(lib, capi, data)[0] != 0 and _snapshot_camera(lib, capi, data)[0] != 0
+        return sm.read_params(lib, capi, data)[0] != 0 and _snapshot_camera(lib, capi, data)[0] != 0
     assert rejected(v3, version=2)                                      # the record is not a version-2 section
     assert rejected(v2, version=3)                                      # version 3 without its record
     assert rejected(v3[:-1]) and rejected(v3 + b"\0")                   # a record of the wrong length
-    assert rejected(_v1_body(capi, lib, p1) + cam)                      # a colourless snapshot has no version 3
+    assert rejected(sm.v1_body(capi, lib, p1) + cam)                    # a colourless snapshot has no version 3
     assert rejected(v3, version=4)
-    for bad in (_camera_bytes(capi, K_=(0.0, 1081.0, 959.5, 539.5)), _camera_bytes(capi, cols=0), _camera_bytes(capi, t=(float("nan"), 0, 0))):
+    for bad in (sm.camera_bytes(capi, K_=(0.0, 1081.0, 959.5, 539.5)), sm.camera_bytes(capi, cols=0), sm.camera_bytes(capi, t=(float("nan"), 0, 0))):
         assert rejected(v2 + bad)                                       # the record obeys df_color_map_dims' rule
     corrupt = bytearray(snap); corrupt[-3] ^= 1                         # the checksum covers the record
-    assert _call(lib, capi, bytes(corrupt))[0] != 0
+    assert sm.read_params(lib, capi, bytes(corrupt))[0] != 0
     out_cam, present = capi.ColorCamera(), C.c_int()
     assert lib.df_kinfu_snapshot_color_camera(np.frombuffer(snap, np.uint8).ctypes.data, len(snap), None, C.byref(present)) == 0 and present.value == 1
     assert lib.df_kinfu_snapshot_color_camera(np.frombuffer(snap, np.uint8).ctypes.data, len(snap), C.byref(out_cam), None) != 0
@@ -239,10 +233,10 @@ def test_snapshot_version_3_checks(lib):
 def test_python_binding_reads_the_camera(lib):
     from dynamicfusion_b200 import capi
     from dynamicfusion_b200.kinfu import COLOR, KinFu
-    p2 = _params(capi, lib, COLOR)
-    length, cls, payload, rgba = _color_sections(tuple(p2.volume_dims))
-    v2 = _v1_body(capi, lib, p2) + length + cls + payload + rgba
-    v3 = v2 + _camera_bytes(capi)
+    p2 = sm.small_params(capi, lib, COLOR)
+    length, cls, payload, rgba = sm.color_sections(tuple(p2.volume_dims))
+    v2 = sm.v1_body(capi, lib, p2) + length + cls + payload + rgba
+    v3 = v2 + sm.camera_bytes(capi)
     cam = KinFu.snapshot_color_camera(sm.header(v3, version=3) + v3)
     assert (cam.cols, cam.rows, cam.intr.fx, cam.depth_to_color.t[0]) == (1920, 1080, 1081.0, np.float32(0.052))
     assert KinFu.snapshot_color_camera(sm.header(v2, version=2) + v2) is None

@@ -19,27 +19,10 @@ import color_camera_oracle as cco  # noqa: E402
 import color_oracle as co  # noqa: E402
 import snapshot_model as sm  # noqa: E402
 from dynamicfusion_b200 import build, capi, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 I3 = np.eye(3, dtype=np.float32)
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _dev(a):
-    a = np.ascontiguousarray(a)
-    view = {np.dtype(np.uint32): np.int32, np.dtype(np.uint16): np.int16}.get(a.dtype)
-    return torch.from_numpy(a.view(view) if view else a).cuda()
-
-
-def _padded(img, extra, fill):
-    """(device tensor with `extra` more elements per row, pitch in bytes, host view with the same strides)"""
-    rows, cols = img.shape[:2]
-    host = np.full((rows, cols + extra) + img.shape[2:], fill, img.dtype)
-    host[:, :cols] = img
-    return _dev(host), host.strides[0], host[:, :cols]
 
 
 def _rot(deg_y):
@@ -74,18 +57,18 @@ def _kernel_case(dims, size, cols, rows, K, depths, cam, pad, cpad, seed=0):
     mc, mr, _ = cco.map_dims(K, cam)
     cs = _cam_struct(cam)
     for depth in depths:
-        d_dev, d_pitch, d_host = _padded(depth, pad, 7)
+        d_dev, d_pitch, d_host = gu.padded(depth, pad, 7)
         dists = torch.zeros((rows, cols + pad), dtype=torch.int16, device="cuda")
-        capi.check(lib.df_compute_dists(d_dev.data_ptr(), d_pitch, cols, rows, intr, dists.data_ptr(), (cols + pad) * 2, _stream()))
+        capi.check(lib.df_compute_dists(d_dev.data_ptr(), d_pitch, cols, rows, intr, dists.data_ptr(), (cols + pad) * 2, gu.stream()))
         capi.check(lib.df_integrate_tracked(V, dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam), intr, None,
-                                            act.data_ptr(), None, _stream()))
+                                            act.data_ptr(), None, gu.stream()))
         cmap = torch.full((mr, mc + cpad), 0x5a5a5a5a, dtype=torch.int32, device="cuda")
-        capi.check(lib.df_color_depth_map(d_dev.data_ptr(), d_pitch, cols, rows, intr, cs, cmap.data_ptr(), (mc + cpad) * 4, _stream()))
+        capi.check(lib.df_color_depth_map(d_dev.data_ptr(), d_pitch, cols, rows, intr, cs, cmap.data_ptr(), (mc + cpad) * 4, gu.stream()))
         img = rng.integers(0, 256, (cam.rows, cam.cols, 4), np.uint8)
-        i_dev, i_pitch, i_host = _padded(img, cpad, 99)
+        i_dev, i_pitch, i_host = gu.padded(img, cpad, 99)
         for colours, a in ((g_tr, act.data_ptr()), (g_de, None)):
             capi.check(lib.df_integrate_color_camera(V, colours.data_ptr(), dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam),
-                                                     intr, cs, i_dev.data_ptr(), i_pitch, cmap.data_ptr(), (mc + cpad) * 4, a, _stream()))
+                                                     intr, cs, i_dev.data_ptr(), i_pitch, cmap.data_ptr(), (mc + cpad) * 4, a, gu.stream()))
         gmap = cmap.cpu().numpy().view(np.uint32)
         assert np.all(gmap[:, mc:] == 0x5a5a5a5a)                      # nothing written past the map's columns
         omap = cco.depth_map(d_host, K, cam)
@@ -136,15 +119,6 @@ def _segment_distance(a, b, c):
     return np.linalg.norm(a + s[..., None] * d - c, axis=-1), s
 
 
-def _params(dim=128, flags=kf.COLOR, cloud_capacity=1_000_000):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = 1024
-    p.cloud_capacity = cloud_capacity
-    p.flags = flags
-    return p
-
-
 def _raw(k, which):
     ptr, pitch, c_, r_ = C.c_void_p(), C.c_size_t(), C.c_int(), C.c_int()
     capi.check(k.lib.df_kinfu_get_buffer(k.h, which, C.byref(ptr), C.byref(pitch), C.byref(c_), C.byref(r_)))
@@ -158,7 +132,7 @@ def test_occlusion_keeps_the_sphere_off_the_wall():
     Kc = (1081.37, 1081.37, 959.5, 539.5)                               # wall behind the small sphere is blocked further out, off the cap
     cam = cco.Camera(1920, 1080, Kc, (I3, (-centre).astype(np.float32)))
     depth, bgra = synth.umbrella_rgbd(0, color_camera=(Kc, 1920, 1080, cam.d2c))
-    k = kf.KinFu(_params())
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     k.set_color_camera(Kc, 1920, 1080, cam.d2c)
     k(depth, bgra)
     loop = k.buffer("color_volume")
@@ -216,19 +190,16 @@ def _with_camera(p, camera=KV2):
     return k
 
 
-def _state(k):
-    return k.state_digest(), [np.concatenate([a.reshape(-1) for a in k.getCameraPose(i)]).tobytes() for i in range(k.info()["poses"])]
-
-
 @pytest.mark.parametrize("extra", [0, kf.LIVE_MODEL, kf.EXTEND_FIELD, kf.RIGID_ONLY], ids=["default", "live_model", "extend_field", "rigid_only"])
 def test_colour_camera_never_feeds_back(extra):
-    plain, colour = kf.KinFu(_params(flags=extra)), _with_camera(_params(flags=extra | kf.COLOR))
+    plain, colour = (kf.KinFu(gu.kinfu_params(128, extra, max_nodes=1024, cloud_capacity=1_000_000)),
+                     _with_camera(gu.kinfu_params(128, extra | kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)))
     for depth, bgra in _frames(6):
         plain(depth)
         colour(depth, bgra)
         first = colour.info()["frame_counter"] == 1
         assert colour.info()["launches"] - plain.info()["launches"] == (3 if not (extra & kf.RIGID_ONLY) or first else 2)
-        assert _state(plain) == _state(colour)
+        assert gu.state(plain) == gu.state(colour)
     assert (colour.buffer("color_volume") >> 24).max() == 6
     if not extra & kf.RIGID_ONLY:
         assert (colour.mesh_colors()[:, 3] == 255).mean() > 0.5
@@ -246,21 +217,21 @@ def _rebuild_frame(k, colours, depth, bgra, cam):
     cs = _cam_struct(cam)
     mc, mr, _ = cco.map_dims(synth.DEFAULT_K, cam)
     cmap = torch.zeros((mr, mc), dtype=torch.int32, device="cuda")
-    d_dev = _dev(depth)
-    capi.check(lib.df_color_depth_map(d_dev.data_ptr(), p.cols * 2, p.cols, p.rows, p.intr, cs, cmap.data_ptr(), mc * 4, _stream()))
+    d_dev = gu.dev(depth)
+    capi.check(lib.df_color_depth_map(d_dev.data_ptr(), p.cols * 2, p.cols, p.rows, p.intr, cs, cmap.data_ptr(), mc * 4, gu.stream()))
     vs = tuple(p.volume_size[i] / p.volume_dims[i] for i in range(3))
     V = capi.make_volume(None, tuple(p.volume_dims), vs, max(p.tsdf_trunc_dist, np.float32(2.1) * np.float32(max(vs))), p.tsdf_max_weight)
     vol_pose = (np.array(p.volume_pose.R, np.float32).reshape(3, 3), np.array(p.volume_pose.t, np.float32))
     vol2cam = co.aff_mul(co.aff_inv(k.getCameraPose()), vol_pose)
     dists, dpitch = dev_ptr(kf.BUF["dists"])
     act, _ = dev_ptr(kf.BUF["activity"])
-    img = _dev(bgra)
+    img = gu.dev(bgra)
     capi.check(lib.df_integrate_color_camera(V, colours.data_ptr(), dists, dpitch, p.cols, p.rows, capi.make_aff(*vol2cam), p.intr, cs, img.data_ptr(),
-                                             cam.cols * 4, cmap.data_ptr(), mc * 4, act, _stream()))
+                                             cam.cols * 4, cmap.data_ptr(), mc * 4, act, gu.stream()))
     cloud, _ = dev_ptr(kf.BUF["cloud"])
     n = k.info()["cloud_points"]
     out = torch.zeros(max(n, 1), dtype=torch.int32, device="cuda")
-    capi.check(lib.df_sample_colors(V, colours.data_ptr(), p.volume_pose, 0.5, cloud, 0, 4, n, 1, None, out.data_ptr(), 0, _stream()))
+    capi.check(lib.df_sample_colors(V, colours.data_ptr(), p.volume_pose, 0.5, cloud, 0, 4, n, 1, None, out.data_ptr(), 0, gu.stream()))
     return cmap.cpu().numpy().view(np.uint32), out[:n].cpu().numpy().view(np.uint8).reshape(-1, 4)
 
 
@@ -270,7 +241,7 @@ def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap):
     cam = cco.Camera(KV2[1], KV2[2], KV2[0], KV2[3])
     runs = []
     for rep in range(2):
-        k = _with_camera(_params())
+        k = _with_camera(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
         mine = torch.zeros(128 ** 3, dtype=torch.int32, device="cuda")
         per_frame = []
         for depth, bgra in _frames(5):
@@ -293,7 +264,9 @@ def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap):
 
 def test_identity_camera_agrees_with_the_registered_path():
     """a colour camera equal to the depth camera: the same pixels, only the occlusion map's coverage differs"""
-    reg, idc = kf.KinFu(_params()), _with_camera(_params(), (synth.DEFAULT_K, 640, 480, (I3, np.zeros(3, np.float32))))
+    reg, idc = (kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)),
+                _with_camera(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000),
+                             (synth.DEFAULT_K, 640, 480, (I3, np.zeros(3, np.float32)))))
     for t in range(6):
         depth, bgra = synth.umbrella_rgbd(t)
         reg(depth, bgra)
@@ -314,7 +287,7 @@ IDENTITY_MIN_SHARE = 0.8
 
 
 def test_texture_fidelity_c2_256_kinect_v2_camera():
-    k = _with_camera(_params(dim=256, cloud_capacity=2_000_000))
+    k = _with_camera(gu.kinfu_params(256, kf.COLOR, max_nodes=1024, cloud_capacity=2_000_000))
     for depth, bgra in _frames(20):
         k(depth, bgra)
     verts, _, faces = k.mesh()
@@ -341,11 +314,11 @@ def test_texture_fidelity_c2_256_kinect_v2_camera():
 # ------------------------------------------------------------------------------------------------------------------------- refusals
 def test_refusals_write_nothing(capfd):
     depth, bgra = _frames(1)[0]
-    plain = kf.KinFu(_params(flags=0))
+    plain = kf.KinFu(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000))
     with pytest.raises(RuntimeError):
         plain.set_color_camera(*KV2)                                    # no colour volume
     plain.close()
-    k = kf.KinFu(_params())
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     with pytest.raises(RuntimeError):
         k.set_color_camera((0.0, 1081.0, 959.5, 539.5), 1920, 1080)     # invalid intrinsics
     with pytest.raises(RuntimeError):
@@ -377,7 +350,7 @@ def test_refusals_write_nothing(capfd):
 
 def test_version_3_resumes_and_rejects(tmp_path, capfd):
     frames = _frames(7)
-    ref = _with_camera(_params(dim=64))
+    ref = _with_camera(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     want, snap = [], None
     for i, (depth, bgra) in enumerate(frames):
         ref(depth, bgra)
@@ -389,8 +362,9 @@ def test_version_3_resumes_and_rejects(tmp_path, capfd):
     assert bytes(kf.KinFu.snapshot_color_camera(snap)) == bytes(_cam_struct(cco.Camera(KV2[1], KV2[2], KV2[0], KV2[3])))
     assert snap[-72:] == bytes(kf.KinFu.snapshot_color_camera(snap))
     # an object without a camera, or with another one, refuses it and keeps its state; a version-2 snapshot is refused by a camera object
-    other = _with_camera(_params(dim=64), (KV2[0], 1920, 1080, (I3, np.array([-0.05, 0.0, 0.0], np.float32))))
-    none = kf.KinFu(_params(dim=64))
+    other = _with_camera(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000),
+                         (KV2[0], 1920, 1080, (I3, np.array([-0.05, 0.0, 0.0], np.float32))))
+    none = kf.KinFu(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     d0, c0 = synth.umbrella_rgbd(0)
     none(d0, c0)
     none_snap = none.snapshot()
@@ -400,7 +374,7 @@ def test_version_3_resumes_and_rejects(tmp_path, capfd):
         with pytest.raises(RuntimeError):
             obj.restore(snap)
         assert (obj.state_digest(), obj.buffer("color_volume").tobytes()) == before
-    fresh = _with_camera(_params(dim=64))
+    fresh = _with_camera(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     with pytest.raises(RuntimeError):
         fresh.restore(none_snap)
     assert "colour camera differs" in capfd.readouterr().err

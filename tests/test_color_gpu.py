@@ -16,28 +16,11 @@ pytestmark = pytest.mark.gpu
 import color_oracle as co  # noqa: E402
 import snapshot_model as sm  # noqa: E402
 from dynamicfusion_b200 import build, capi, kinfu as kf, synth  # noqa: E402
-from test_raster import look_at, sphere_mesh  # noqa: E402
+import gpu_util as gu  # noqa: E402
+from scenes import look_at, sphere_mesh  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 PARAMS_BYTES = C.sizeof(capi.KinfuParams)
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _dev(a):
-    a = np.ascontiguousarray(a)
-    view = {np.dtype(np.uint32): np.int32, np.dtype(np.uint16): np.int16}.get(a.dtype)
-    return torch.from_numpy(a.view(view) if view else a).cuda()
-
-
-def _padded(img, extra, fill):
-    """(device tensor with `extra` more elements per row, pitch in bytes, host view with the same strides)"""
-    rows, cols = img.shape[:2]
-    host = np.full((rows, cols + extra) + img.shape[2:], fill, img.dtype)
-    host[:, :cols] = img
-    return _dev(host), host.strides[0], host[:, :cols]
 
 
 def _random_bgra(rng, rows, cols):
@@ -64,16 +47,16 @@ def _integrate_case(dims, size, cols, rows, depths, pad=0, seed=0):
     o_tr, o_de = np.zeros(nvox, np.uint32), np.zeros(nvox, np.uint32)
     visited = []
     for depth in depths:
-        d_dev, d_pitch, _ = _padded(depth, pad, 0)
+        d_dev, d_pitch, _ = gu.padded(depth, pad, 0)
         dists = torch.zeros((rows, cols + pad), dtype=torch.int16, device="cuda")
-        capi.check(lib.df_compute_dists(d_dev.data_ptr(), d_pitch, cols, rows, intr, dists.data_ptr(), (cols + pad) * 2, _stream()))
+        capi.check(lib.df_compute_dists(d_dev.data_ptr(), d_pitch, cols, rows, intr, dists.data_ptr(), (cols + pad) * 2, gu.stream()))
         capi.check(lib.df_integrate_tracked(V, dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam), intr, None,
-                                            act.data_ptr(), None, _stream()))
+                                            act.data_ptr(), None, gu.stream()))
         img = _random_bgra(rng, rows, cols)
-        i_dev, i_pitch, i_host = _padded(img, pad, 99)
+        i_dev, i_pitch, i_host = gu.padded(img, pad, 99)
         for colours, a in ((g_tr, act.data_ptr()), (g_de, None)):
             capi.check(lib.df_integrate_color(V, colours.data_ptr(), dists.data_ptr(), (cols + pad) * 2, i_dev.data_ptr(), i_pitch, cols, rows,
-                                              capi.make_aff(*vol2cam), intr, a, _stream()))
+                                              capi.make_aff(*vol2cam), intr, a, gu.stream()))
         dists_host = dists.cpu().numpy().view(np.uint16)[:, :cols]
         act_host = act.cpu().numpy()
         co.integrate_color(o_tr, dims, vs, trunc, 64, dists_host, i_host, vol2cam, K, act_host)
@@ -108,12 +91,12 @@ def _gpu_sample(colours, dims, vs, pose, offset, pts, count=None):
     P = np.ascontiguousarray(pts, np.float32)
     rows, cols = (1, len(P)) if P.ndim == 2 else P.shape[:2]
     stride = P.shape[-1]
-    pd = _dev(P)
+    pd = gu.dev(P)
     out = torch.full((rows, cols), 0x01010101, dtype=torch.int32, device="cuda")
     cnt = None if count is None else torch.tensor([count], dtype=torch.int32, device="cuda")
     V = capi.make_volume(None, dims, vs, 0.04, 64)
-    capi.check(lib.df_sample_colors(V, _dev(colours).data_ptr(), capi.make_aff(*pose), offset, pd.data_ptr(), cols * stride * 4, stride, cols, rows,
-                                    None if cnt is None else cnt.data_ptr(), out.data_ptr(), cols * 4, _stream()))
+    capi.check(lib.df_sample_colors(V, gu.dev(colours).data_ptr(), capi.make_aff(*pose), offset, pd.data_ptr(), cols * stride * 4, stride, cols, rows,
+                                    None if cnt is None else cnt.data_ptr(), out.data_ptr(), cols * 4, gu.stream()))
     return out.cpu().numpy().view(np.uint8).reshape(P.shape[:-1] + (4,))
 
 
@@ -151,7 +134,7 @@ def test_sample_colors_equals_the_oracle():
 # ---------------------------------------------------------------------------------------------------------------- df_mesh_colors
 def _gpu_raster(verts, tris, w2c, K, cols, rows):
     lib = capi.load()
-    v, t = _dev(np.asarray(verts, np.float32)), _dev(np.asarray(tris, np.int32).reshape(-1, 3))
+    v, t = gu.dev(np.asarray(verts, np.float32)), gu.dev(np.asarray(tris, np.int32).reshape(-1, 3))
     pts = torch.empty((rows, cols, 4), dtype=torch.float32, device="cuda")
     nrm = torch.empty_like(pts)
     ids = torch.empty((rows, cols), dtype=torch.int32, device="cuda")
@@ -159,16 +142,16 @@ def _gpu_raster(verts, tris, w2c, K, cols, rows):
     ws = torch.empty(lib.df_raster_workspace_bytes(len(v), len(t), cols, rows), dtype=torch.uint8, device="cuda")
     capi.check(lib.df_raster_mesh(v.data_ptr(), len(v), v.shape[1], t.data_ptr(), len(t), capi.make_aff(*w2c), capi.make_intr(*K), cols, rows,
                                   ids.data_ptr(), cols * 4, pts.data_ptr(), cols * 16, nrm.data_ptr(), cols * 16, stats.data_ptr(), ws.data_ptr(),
-                                  _stream()))
+                                  gu.stream()))
     return v, t, ids, pts, stats.cpu().numpy()
 
 
 def _gpu_mesh_colors(v, t, ids, pts, w2c, rgba, cols, rows, pad=3):
     lib = capi.load()
     img = torch.full((rows, cols + pad, 4), 77, dtype=torch.uint8, device="cuda")
-    c = _dev(np.ascontiguousarray(rgba).view(np.uint32).reshape(-1))
+    c = gu.dev(np.ascontiguousarray(rgba).view(np.uint32).reshape(-1))
     capi.check(lib.df_mesh_colors(ids.data_ptr(), cols * 4, pts.data_ptr(), cols * 16, v.data_ptr(), len(v), v.shape[1], t.data_ptr(), len(t),
-                                  capi.make_aff(*w2c), c.data_ptr(), cols, rows, img.data_ptr(), (cols + pad) * 4, _stream()))
+                                  capi.make_aff(*w2c), c.data_ptr(), cols, rows, img.data_ptr(), (cols + pad) * 4, gu.stream()))
     out = img.cpu().numpy()
     assert np.all(out[:, cols:] == 77)                                  # nothing past the image's columns
     return out[:, :cols]
@@ -193,30 +176,18 @@ def test_mesh_colors_equals_the_oracle_on_the_sphere():
 
 
 # ------------------------------------------------------------------------------------------------------------------- the frame loop
-def _params(dim=128, flags=kf.COLOR, cloud_capacity=1_000_000):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = 1024
-    p.cloud_capacity = cloud_capacity
-    p.flags = flags
-    return p
-
-
 RGBD = [synth.umbrella_rgbd(t) for t in range(8)]
-
-
-def _state(k):
-    return k.state_digest(), [np.concatenate([a.reshape(-1) for a in k.getCameraPose(i)]).tobytes() for i in range(k.info()["poses"])]
 
 
 @pytest.mark.parametrize("extra", [0, kf.LIVE_MODEL, kf.EXTEND_FIELD, kf.RIGID_ONLY], ids=["default", "live_model", "extend_field", "rigid_only"])
 def test_colour_never_feeds_back(extra):
-    plain, colour = kf.KinFu(_params(flags=extra)), kf.KinFu(_params(flags=extra | kf.COLOR))
+    plain, colour = (kf.KinFu(gu.kinfu_params(128, extra, max_nodes=1024, cloud_capacity=1_000_000)),
+                     kf.KinFu(gu.kinfu_params(128, extra | kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)))
     for depth, bgra in RGBD[:6]:
         plain(depth)
         colour(depth, bgra)
         assert colour.info()["launches"] - plain.info()["launches"] == (2 if not (extra & kf.RIGID_ONLY) or colour.info()["frame_counter"] == 1 else 1)
-        assert _state(plain) == _state(colour)
+        assert gu.state(plain) == gu.state(colour)
     assert (colour.buffer("color_volume") >> 24).max() == 6
     if not extra & kf.RIGID_ONLY:
         assert (colour.mesh_colors()[:, 3] == 255).mean() > 0.5
@@ -237,13 +208,13 @@ def _rebuild_frame(k, colours, bgra):
     vol2cam = co.aff_mul(co.aff_inv(k.getCameraPose()), vol_pose)
     dists, dpitch = dev_ptr(kf.BUF["dists"])
     act, _ = dev_ptr(kf.BUF["activity"])
-    img = _dev(bgra)
+    img = gu.dev(bgra)
     capi.check(lib.df_integrate_color(V, colours.data_ptr(), dists, dpitch, img.data_ptr(), p.cols * 4, p.cols, p.rows, capi.make_aff(*vol2cam),
-                                      p.intr, act, _stream()))
+                                      p.intr, act, gu.stream()))
     cloud, _ = dev_ptr(kf.BUF["cloud"])
     n = k.info()["cloud_points"]
     out = torch.zeros(max(n, 1), dtype=torch.int32, device="cuda")
-    capi.check(lib.df_sample_colors(V, colours.data_ptr(), p.volume_pose, 0.5, cloud, 0, 4, n, 1, None, out.data_ptr(), 0, _stream()))
+    capi.check(lib.df_sample_colors(V, colours.data_ptr(), p.volume_pose, 0.5, cloud, 0, 4, n, 1, None, out.data_ptr(), 0, gu.stream()))
     return out[:n].cpu().numpy().view(np.uint8).reshape(-1, 4)
 
 
@@ -252,7 +223,7 @@ def test_loop_colours_rebuilt_from_the_public_entries(monkeypatch, overlap):
     monkeypatch.setenv("DF_KINFU_OVERLAP_EXTRACT", overlap)
     runs = []
     for rep in range(2):
-        k = kf.KinFu(_params())
+        k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
         mine = torch.zeros(128 ** 3, dtype=torch.int32, device="cuda")
         per_frame = []
         for depth, bgra in RGBD[:5]:
@@ -278,9 +249,9 @@ def test_loop_colours_rebuilt_from_the_public_entries(monkeypatch, overlap):
 
 def test_refusals(capfd):
     with pytest.raises(RuntimeError):
-        kf.KinFu(_params(flags=kf.COLOR | kf.WARPED_INTEGRATE))
+        kf.KinFu(gu.kinfu_params(128, kf.COLOR | kf.WARPED_INTEGRATE, max_nodes=1024, cloud_capacity=1_000_000))
     assert "DF_KINFU_WARPED_INTEGRATE" in capfd.readouterr().err
-    k = kf.KinFu(_params(flags=0))
+    k = kf.KinFu(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000))
     depth, bgra = RGBD[0]
     with pytest.raises(RuntimeError):
         k(depth, bgra)
@@ -291,8 +262,8 @@ def test_refusals(capfd):
         with pytest.raises(RuntimeError):
             call()
     k.close()
-    k = kf.KinFu(_params())                                             # device frames give what host frames give
-    h = kf.KinFu(_params())
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))  # device frames give what host frames give
+    h = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     for depth, bgra in RGBD[:3]:
         k(torch.from_numpy(depth.view(np.int16)).cuda(), torch.from_numpy(bgra).cuda())
         h(depth, bgra)
@@ -302,7 +273,7 @@ def test_refusals(capfd):
 
 # ------------------------------------------------------------------------------------------------------------------------ fidelity
 def test_texture_fidelity_c2_256(tmp_path):
-    k = kf.KinFu(_params(dim=256, cloud_capacity=2_000_000))
+    k = kf.KinFu(gu.kinfu_params(256, kf.COLOR, max_nodes=1024, cloud_capacity=2_000_000))
     for t in range(20):
         k(*synth.umbrella_rgbd(t))
     verts, _, faces = k.mesh()
@@ -342,7 +313,7 @@ FIDELITY_MIN_FRACTION, FIDELITY_MEDIAN, FIDELITY_P90 = 0.9, 20.0, 75.0
 
 # ----------------------------------------------------------------------------------------------------------------------- snapshots
 def test_colourless_snapshot_is_version_1():
-    k = kf.KinFu(_params(dim=64, flags=0))
+    k = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=1024, cloud_capacity=1_000_000))
     for depth, _ in RGBD[:3]:
         k(depth)
     snap = k.snapshot()
@@ -356,7 +327,7 @@ def test_colourless_snapshot_is_version_1():
 
 def test_version_2_resumes_and_rejects(capfd):
     frames = RGBD[:7]
-    ref = kf.KinFu(_params(dim=64))
+    ref = kf.KinFu(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     want, snap = [], None
     for i, (depth, bgra) in enumerate(frames):
         ref(depth, bgra)
@@ -367,7 +338,7 @@ def test_version_2_resumes_and_rejects(capfd):
     assert struct.unpack_from("<I", snap, 8)[0] == 2
     n_cloud = sm.counters(snap, PARAMS_BYTES)[4]
     assert kf.KinFu.snapshot_params(snap).flags & kf.COLOR
-    k = kf.KinFu(_params(dim=64))
+    k = kf.KinFu(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     k(*frames[0])
     before = (k.state_digest(), k.buffer("color_volume").tobytes(), k.buffer("cloud_colors").tobytes())
     # damaged colour sections are refused with the state unchanged
@@ -392,7 +363,7 @@ def test_version_2_resumes_and_rejects(capfd):
             k.restore(b)
         assert (k.state_digest(), k.buffer("color_volume").tobytes(), k.buffer("cloud_colors").tobytes()) == before
     assert "rejected" in capfd.readouterr().err
-    plain = kf.KinFu(_params(dim=64, flags=0))
+    plain = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=1024, cloud_capacity=1_000_000))
     with pytest.raises(RuntimeError):
         plain.restore(snap)                                             # other parameters
     plain.close()
@@ -406,7 +377,7 @@ def test_version_2_resumes_and_rejects(capfd):
 
 # --------------------------------------------------------------------------------------------------------------------------- hosts
 def test_render_image_flag_4_is_mesh_colors_of_the_render():
-    k = kf.KinFu(_params())
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     for depth, bgra in RGBD[:6]:
         k(depth, bgra)
     digest = k.state_digest()

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 torch = pytest.importorskip("torch")
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("orc")]
 
 import color_camera_oracle as cco  # noqa: E402
 import color_oracle as co  # noqa: E402
@@ -21,21 +21,13 @@ import color_track_reference as ctr  # noqa: E402
 import icp_cases as ic  # noqa: E402
 import icp_reference as ir  # noqa: E402
 from dynamicfusion_b200 import build, capi, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 SCRATCH = 32 + 27 * 1024
 W, MAXR = capi.COLOR_TRACK_WEIGHT, capi.COLOR_TRACK_MAX_RESIDUAL
 KV2 = ((1620.0, 1620.0, 959.5, 539.5), 1920, 1080)                   # a Kinect-v2-like colour camera, 52 mm beside the depth camera
 D2C = (np.eye(3, dtype=np.float32), np.array([-0.052, 0.0, 0.0], np.float32))
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _oracle(orc):
-    return orc
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _pad(a, extra, fill):
@@ -65,17 +57,9 @@ def _gpu_frame_intensity(bgra, levels, cols, rows, cam=None, K=None, points=None
     capi.check(capi.load().df_frame_intensity(img.data_ptr(), bp, None if camst is None else C.byref(camst), capi.make_intr(*(K or (1, 1, 0, 0))),
                                               args[0], args[1], args[2], args[3], float(trunc), levels,
                                               _arr(C.c_int, [c for c, _ in sizes]), _arr(C.c_int, [r for _, r in sizes]),
-                                              _arr(C.c_void_p, [o.data_ptr() for o, _ in outs]), _arr(C.c_size_t, [p for _, p in outs]), _stream()))
+                                              _arr(C.c_void_p, [o.data_ptr() for o, _ in outs]), _arr(C.c_size_t, [p for _, p in outs]), gu.stream()))
     torch.cuda.synchronize()
     return [o.cpu().numpy()[:, :c] for (o, _), (c, r) in zip(outs, sizes)]
-
-
-def _same(a, b):
-    """equal bit for bit where a value is, NaN at the same places (the device's NaN and C's NAN differ in their payload bits)"""
-    if a.shape != b.shape:
-        return False
-    nan = np.isnan(a)
-    return np.array_equal(nan, np.isnan(b)) and np.array_equal(a[~nan].view(np.uint32), b[~nan].view(np.uint32))
 
 
 @pytest.mark.parametrize("cols,rows,pad", [(640, 480, 0), (203, 151, 5)])
@@ -84,7 +68,7 @@ def test_frame_intensity_registered(cols, rows, pad):
     bgra = rng.integers(0, 256, (rows, cols, 4), dtype=np.uint8)
     got = _gpu_frame_intensity(bgra, 4, cols, rows, pad=pad)
     want = cto.frame_intensity(bgra, 4)
-    assert all(_same(g, w) for g, w in zip(got, want))
+    assert all(gu.same_bits(g, w) for g, w in zip(got, want))
 
 
 def test_frame_intensity_through_the_colour_camera():
@@ -96,7 +80,7 @@ def test_frame_intensity_through_the_colour_camera():
     cmap = cco.depth_map(depth, K, cam)
     got = _gpu_frame_intensity(bgra, 3, 640, 480, cam=cam, K=K, points=pts, cmap=cmap, trunc=0.04, pad=3)
     want = cto.frame_intensity(bgra, 3, camera=cam, K_depth=K, points=pts, color_map=cmap, trunc_dist=0.04)
-    assert all(_same(g, w) for g, w in zip(got, want))
+    assert all(gu.same_bits(g, w) for g, w in zip(got, want))
     no_occl = cto.frame_intensity(bgra, 1, camera=cam, K_depth=K, points=pts, color_map=np.full_like(cmap, 0x7f000000), trunc_dist=0.04)[0]
     occluded = np.isnan(want[0]) & ~np.isnan(no_occl) & ~np.isnan(pts[..., 0])
     assert occluded.sum() > 50                                      # the small sphere hides part of the wall from the colour camera
@@ -123,7 +107,7 @@ def _gpu_model(colors, dims, vs, cam2vol, pyr, pad=0):
     capi.check(capi.load().df_model_intensity(V, cols_.data_ptr(), capi.make_aff(*cam2vol), L, _arr(C.c_int, [p.shape[1] for p in pyr]),
                                               _arr(C.c_int, [p.shape[0] for p in pyr]), _arr(C.c_void_p, [t.data_ptr() for t, _ in pts]),
                                               _arr(C.c_size_t, [q for _, q in pts]), _arr(C.c_void_p, [t.data_ptr() for t, _ in outs]),
-                                              _arr(C.c_size_t, [q for _, q in outs]), _stream()))
+                                              _arr(C.c_size_t, [q for _, q in outs]), gu.stream()))
     torch.cuda.synchronize()
     return [t.cpu().numpy()[:, :p.shape[1]] for (t, _), p in zip(outs, pyr)]
 
@@ -141,7 +125,7 @@ def test_model_intensity_equals_the_oracle(scene):
         cam2vol = co.aff_mul(co.aff_inv(vol_pose), tuple(np.asarray(x, np.float32) for x in P))
         got = _gpu_model(colors, dims, vs, cam2vol, pyr, pad=2)
         want = [cto.model_intensity(colors, dims, vs, cam2vol, p) for p in pyr]
-        assert all(_same(g, w) for g, w in zip(got, want))
+        assert all(gu.same_bits(g, w) for g, w in zip(got, want))
         assert (~np.isnan(want[0][..., 0])).mean() > 0.3
 
 
@@ -152,7 +136,7 @@ def _gpu_accumulate_color(curr, prev, icurr, model, K, T, dist2, min_cos, weight
     rows, cols = icurr.shape
     args = [x for t, p in maps for x in (t.data_ptr(), p)]
     capi.check(capi.load().df_icp_accumulate_color(*args, cols, rows, capi.make_intr(*K), capi.make_aff(*T), float(dist2), float(min_cos),
-                                                   float(weight), float(MAXR), scratch.data_ptr(), _stream()))
+                                                   float(weight), float(MAXR), scratch.data_ptr(), gu.stream()))
     torch.cuda.synchronize()
     return scratch.cpu().numpy()
 
@@ -163,7 +147,7 @@ def _gpu_accumulate(curr, prev, K, T, dist2, min_cos):
     rows, cols = curr[0].shape[:2]
     args = [x for t, p in maps for x in (t.data_ptr(), p)]
     capi.check(capi.load().df_icp_accumulate(*args, cols, rows, capi.make_intr(*K), capi.make_aff(*T), float(dist2), float(min_cos),
-                                             scratch.data_ptr(), _stream()))
+                                             scratch.data_ptr(), gu.stream()))
     torch.cuda.synchronize()
     return scratch.cpu().numpy()
 
@@ -222,7 +206,7 @@ def _gpu_estimate_color(P, iters, pad=0):
                                                  ptrs(mm), _arr(C.c_size_t, [p for _, p in mm]), _arr(C.c_int, [c[0].shape[1] for c in curr]),
                                                  _arr(C.c_int, [c[0].shape[0] for c in curr]), _arr(C.c_size_t, [p for _, p in vc]), L,
                                                  _arr(C.c_int, list(iters)), capi.make_intr(*P["K"]), float(ctr.DIST), float(ctr.ANGLE),
-                                                 float(W), float(MAXR), T.data_ptr(), ok.data_ptr(), scratch.data_ptr(), _stream()))
+                                                 float(W), float(MAXR), T.data_ptr(), ok.data_ptr(), scratch.data_ptr(), gu.stream()))
     torch.cuda.synchronize()
     t = T.cpu().numpy()
     return bool(ok.cpu().numpy()[0]), (t[:9].reshape(3, 3).copy(), t[9:12].copy()), scratch.cpu().numpy()
@@ -257,26 +241,13 @@ def test_estimate_color_every_step_against_step64(scene, request):
 
 
 # ------------------------------------------------------------------------------------------------------------ the frame loop
-def _params(dim=256, flags=kf.COLOR | kf.COLOR_TRACKING):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = 1024
-    p.cloud_capacity = 1_000_000
-    p.flags = flags
-    return p
-
-
-def _state(k):
-    return k.state_digest(), [np.concatenate([a.reshape(-1) for a in k.getCameraPose(i)]).tobytes() for i in range(k.info()["poses"])]
-
-
 WALL = [synth.textured_wall_rgbd(t) for t in range(21)]
 
 
 @pytest.mark.parametrize("overlap", ["1", "0"])
 def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap):
     monkeypatch.setenv("DF_KINFU_OVERLAP_EXTRACT", overlap)
-    k = kf.KinFu(_params(128))
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR | kf.COLOR_TRACKING, max_nodes=1024, cloud_capacity=1_000_000))
     p = k.params
     K = (p.intr.fx, p.intr.fy, p.intr.cx, p.intr.cy)
     vs = (1.0 / 128,) * 3
@@ -290,9 +261,9 @@ def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap):
         curr = [(k.buffer("curr_points", l), k.buffer("curr_normals", l)) for l in range(3)]
         icurr = [k.buffer("intensity", l) for l in range(3)]
         model = [k.buffer("model_intensity", l) for l in range(3)]
-        assert all(_same(a, b) for a, b in zip(icurr, cto.frame_intensity(WALL[t][1], 3)))
+        assert all(gu.same_bits(a, b) for a, b in zip(icurr, cto.frame_intensity(WALL[t][1], 3)))
         cam2vol = co.aff_mul(co.aff_inv(vol_pose), pose_prev)
-        assert all(_same(m, cto.model_intensity(colors, (128,) * 3, vs, cam2vol, pv[0])) for m, pv in zip(model, prev))
+        assert all(gu.same_bits(m, cto.model_intensity(colors, (128,) * 3, vs, cam2vol, pv[0])) for m, pv in zip(model, prev))
         ok, T, _ = _gpu_estimate_color(dict(curr=curr, prev=prev, icurr=icurr, model=model, K=K), list(p.icp_iter_num)[:3])
         assert ok
         pose = co.aff_mul(pose_prev, T)
@@ -302,14 +273,16 @@ def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap):
 
 
 def test_depth_only_frames_and_launch_counts():
-    a, b = kf.KinFu(_params(128, kf.COLOR)), kf.KinFu(_params(128))
+    a, b = (kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)),
+            kf.KinFu(gu.kinfu_params(128, kf.COLOR | kf.COLOR_TRACKING, max_nodes=1024, cloud_capacity=1_000_000)))
     for t in range(4):                                                # depth-only frames: the same state, the same launches
         a(WALL[t][0]); b(WALL[t][0])
-        assert _state(a) == _state(b) and a.info()["launches"] == b.info()["launches"]
+        assert gu.state(a) == gu.state(b) and a.info()["launches"] == b.info()["launches"]
     a.close(); b.close()
     # colour frames of C2, which geometry tracks too (so both runs take the same branches): the pyramid (3 levels) and, after the first
     # frame, the model maps
-    a, b = kf.KinFu(_params(128, kf.COLOR)), kf.KinFu(_params(128))
+    a, b = (kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)),
+            kf.KinFu(gu.kinfu_params(128, kf.COLOR | kf.COLOR_TRACKING, max_nodes=1024, cloud_capacity=1_000_000)))
     for t in range(4):
         d, c = synth.umbrella_rgbd(t)
         a(d, c); b(d, c)
@@ -322,7 +295,7 @@ def test_depth_only_frames_and_launch_counts():
 
 
 def _run_sequence(frames, truth, flags, dim=256, cam=None):
-    k = kf.KinFu(_params(dim, flags))
+    k = kf.KinFu(gu.kinfu_params(dim, flags, max_nodes=1024, cloud_capacity=1_000_000))
     if cam is not None:
         k.set_color_camera(*cam)
     errs = []
@@ -369,20 +342,20 @@ def test_c2_rgbd_is_tracked():
 
 def test_snapshot_resume_equals_the_uninterrupted_run():
     frames = WALL[:10]
-    k = kf.KinFu(_params(128))
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR | kf.COLOR_TRACKING, max_nodes=1024, cloud_capacity=1_000_000))
     states = []
     snap = None
     for t, f in enumerate(frames):
         k(*f)
-        states.append(_state(k))
+        states.append(gu.state(k))
         if t == 4:
             snap = k.snapshot()
     k.close()
-    r = kf.KinFu(_params(128))
+    r = kf.KinFu(gu.kinfu_params(128, kf.COLOR | kf.COLOR_TRACKING, max_nodes=1024, cloud_capacity=1_000_000))
     r.restore(snap)
     for t in range(5, 10):
         r(*frames[t])
-        assert _state(r) == states[t]
+        assert gu.state(r) == states[t]
     r.close()
 
 
@@ -390,10 +363,11 @@ def test_refusals_and_the_environment(capfd, monkeypatch):
     for flags, word in ((kf.COLOR_TRACKING, "DF_KINFU_COLOR"), (kf.COLOR | kf.COLOR_TRACKING | kf.USE_DEPTH, "DF_KINFU_USE_DEPTH"),
                         (kf.COLOR | kf.COLOR_TRACKING | kf.LIVE_MODEL, "DF_KINFU_LIVE_MODEL")):
         with pytest.raises(RuntimeError):
-            kf.KinFu(_params(128, flags))
+            kf.KinFu(gu.kinfu_params(128, flags, max_nodes=1024, cloud_capacity=1_000_000))
         assert word in capfd.readouterr().err
     monkeypatch.setenv("DF_KINFU_COLOR_TRACKING", "1")
-    k, plain = kf.KinFu(_params(128, kf.COLOR)), kf.KinFu(_params(128, 0))
+    k, plain = (kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)),
+                kf.KinFu(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000)))
     k(*WALL[0]); plain(WALL[0][0])
     assert k.buffer("intensity").shape == (480, 640)                    # the flag is on
     with pytest.raises(RuntimeError):

@@ -8,29 +8,15 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import host, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 K = synth.DEFAULT_K
-
-
-def _params(dim, flags=0, max_nodes=2048, cols=640, rows=480, K_=K):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = max_nodes
-    p.cloud_capacity = 4_000_000
-    p.flags = flags
-    p.cols, p.rows = cols, rows
-    p.intr.fx, p.intr.fy, p.intr.cx, p.intr.cy = K_
-    return p
-
-
-def _tsdf(vol):
-    return (vol & 0xffff).astype(np.uint16).view(np.float16).astype(np.float32), vol >> 16
 
 
 def test_c1_256_rigid_single_frame(orc):
     """configs[0]: one 640x480 frame into a 256^3 volume, rigid-only integrate + ray-cast: bit-exact (no expf on this path)"""
     from oracle import orc_pipe
-    p = _params(256, kf.RIGID_ONLY)
+    p = gu.kinfu_params(256, kf.RIGID_ONLY, max_nodes=2048, cloud_capacity=4_000_000, K=K, cols=640, rows=480)
     gpu, cpu = kf.KinFu(p), orc_pipe.KinFu(orc_pipe.params_from(p))
     d = synth.sphere_wall_depth(seed=11)
     assert gpu(d) is False and cpu(d) is False
@@ -41,8 +27,8 @@ def test_c1_256_rigid_single_frame(orc):
     Rg, tg = gpu.getCameraPose(1)
     Rc, tc = cpu.getCameraPose(1)
     assert np.abs(Rg - Rc).max() < 2e-4 and np.abs(tg - tc).max() < 2e-4
-    fg, wg = _tsdf(gpu.buffer("volume"))
-    fc, wc = _tsdf(cpu.buffer("volume"))
+    fg, wg = gu.tsdf(gpu.buffer("volume"))
+    fc, wc = gu.tsdf(cpu.buffer("volume"))
     assert np.mean(wg != wc) < 2e-3
     same = wg == wc
     assert np.mean(np.abs(fg[same] - fc[same]) > 2e-3) < 2e-3
@@ -56,7 +42,7 @@ def test_c1_256_rigid_single_frame(orc):
 def test_c3_512_4k_nodes_five_lm_iterations(orc):
     """configs[2]: 512^3, 4k warp nodes, k = 8 DQB, 5 LM iterations per frame -- three frames against the oracle's loop"""
     from oracle import orc_pipe
-    p = _params(512, 0, max_nodes=4096)
+    p = gu.kinfu_params(512, 0, max_nodes=4096, cloud_capacity=4_000_000, K=K, cols=640, rows=480)
     p.solver_nonlinear_iters = 5
     gpu, cpu = kf.KinFu(p), orc_pipe.KinFu(orc_pipe.params_from(p))
     for t in range(3):
@@ -75,8 +61,8 @@ def test_c3_512_4k_nodes_five_lm_iterations(orc):
     assert np.median(np.abs(tg - tc)) <= 5e-3 * scale + 2e-6
     sg, sc = gpu.buffer("solve_stats"), cpu.buffer("solve_stats")
     assert abs(sg[3] - sc[3]) <= 0.01 * sc[3] and abs(sg[1] - sc[1]) <= 5e-2 * sc[1]
-    fg, wg = _tsdf(gpu.buffer("volume"))
-    fc, wc = _tsdf(cpu.buffer("volume"))
+    fg, wg = gu.tsdf(gpu.buffer("volume"))
+    fc, wc = gu.tsdf(cpu.buffer("volume"))
     assert np.mean(wg != wc) < 2e-2
     gpu.close(); cpu.close()
 
@@ -131,7 +117,7 @@ def test_c4_768_hd_full_loop_two_frames(orc):
     from oracle import orc_pipe
     cols, rows = 1280, 720
     K_hd = (K[0] * 2, K[1] * 2, 640.0, 360.0)
-    p = _params(768, 0, max_nodes=2048, cols=cols, rows=rows, K_=K_hd)
+    p = gu.kinfu_params(768, 0, max_nodes=2048, cloud_capacity=4_000_000, K=K_hd, cols=cols, rows=rows)
     for i in range(3):
         p.volume_size[i] = 1.5
     p.volume_pose.t[0] = -0.75; p.volume_pose.t[1] = -0.75; p.volume_pose.t[2] = 0.5
@@ -146,8 +132,8 @@ def test_c4_768_hd_full_loop_two_frames(orc):
     Rg, tg = gpu.getCameraPose(1)
     Rc, tc = cpu.getCameraPose(1)
     assert np.abs(Rg - Rc).max() < 2e-4 and np.abs(tg - tc).max() < 2e-4
-    fg, wg = _tsdf(gpu.buffer("volume"))
-    fc, wc = _tsdf(cpu.buffer("volume"))
+    fg, wg = gu.tsdf(gpu.buffer("volume"))
+    fc, wc = gu.tsdf(cpu.buffer("volume"))
     assert np.mean(wg != wc) < 2e-2
     sg, sc = gpu.buffer("solve_stats"), cpu.buffer("solve_stats")
     assert abs(sg[3] - sc[3]) <= 0.01 * sc[3] and abs(sg[1] - sc[1]) <= 5e-2 * sc[1]

@@ -10,7 +10,7 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import host  # noqa: E402
-from test_f2_oracle import _patch, _rot_y  # noqa: E402
+from scenes import node_patch, rot_y  # noqa: E402
 
 
 def _run_both(orc, node_pts, src, dst, weight, **kw):
@@ -25,9 +25,9 @@ def _run_both(orc, node_pts, src, dst, weight, **kw):
 @pytest.mark.parametrize("flags,lam", [(0, 0.0), (1, 0.0), (1, 2.0), (1 | 4, 2.0), (1 | 2, 0.0), (7, 5.0)])
 def test_f2_matches_oracle(orc, flags, lam):
     rng = np.random.default_rng(17 + flags)
-    node_pts, src = _patch(rng, 6000)
+    node_pts, src = node_patch(rng, 6000)
     dst = src.copy()
-    dst[:, :3] = (src[:, :3] @ _rot_y(3.0).T + np.array([0.008, -0.002, 0.004])).astype(np.float32)
+    dst[:, :3] = (src[:, :3] @ rot_y(3.0).T + np.array([0.008, -0.002, 0.004])).astype(np.float32)
     dst[:, 2] += (0.004 * np.sin(9 * src[:, 1])).astype(np.float32)
     out = rng.choice(len(src), len(src) // 20, replace=False)
     dst[out, :3] += rng.uniform(0.05, 0.2, (len(out), 3)).astype(np.float32)
@@ -58,7 +58,7 @@ def test_f2_full_size_properties():
     src = np.zeros((N, 4), np.float32)
     src[:, 0] = rng.uniform(-0.4, 0.4, N); src[:, 1] = rng.uniform(-0.3, 0.3, N); src[:, 2] = 1.0 + 0.03 * np.sin(7 * src[:, 0])
     dst = src.copy()
-    dst[:, :3] = (src[:, :3] @ _rot_y(2.0).T + np.array([0.004, 0.0, 0.002])).astype(np.float32)
+    dst[:, :3] = (src[:, :3] @ rot_y(2.0).T + np.array([0.004, 0.0, 0.002])).astype(np.float32)
     e = {}
     for flags in (0, 7):
         n = np.zeros((M, 12), np.float32); n[:, :3] = node_pts; n[:, 3] = 1; n[:, 7] = 1; n[:, 11] = 0.05

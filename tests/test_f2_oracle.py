@@ -4,18 +4,7 @@ to the reference-behaviour solver it must reduce to."""
 import numpy as np
 import pytest
 
-
-def _patch(rng, n=2500):
-    gx, gy = np.meshgrid(np.linspace(-0.3, 0.3, 10), np.linspace(-0.2, 0.2, 6))
-    node_pts = np.stack([gx.ravel(), gy.ravel(), np.full(gx.size, 1.0)], 1).astype(np.float32)
-    src = np.zeros((n, 4), np.float32)
-    src[:, 0] = rng.uniform(-0.3, 0.3, n); src[:, 1] = rng.uniform(-0.2, 0.2, n); src[:, 2] = 1.0 + 0.02 * np.sin(8 * src[:, 0])
-    return node_pts, src
-
-
-def _rot_y(deg):
-    a = np.deg2rad(deg)
-    return np.array([[np.cos(a), 0, np.sin(a)], [0, 1, 0], [-np.sin(a), 0, np.cos(a)]])
+from scenes import node_patch, rot_y
 
 
 def test_penalties_are_the_references(orc):
@@ -35,7 +24,7 @@ def test_penalties_are_the_references(orc):
 def test_translation_only_reduces_to_the_data_term_solve(orc):
     """flags = 0, lambda = 0: the energy is the reference-behaviour cost (1/2 sum r^2) and the minimiser is the data-term solve's"""
     rng = np.random.default_rng(5)
-    node_pts, src = _patch(rng)
+    node_pts, src = node_patch(rng)
     dst = src.copy(); dst[:, :3] += np.array([0.01, -0.004, 0.006], np.float32)
     a = orc.make_nodes(node_pts, weight=0.08); b = a.copy()
     st = orc.solve_f2(a, src, dst, orc.f2_params(flags=0, gn_iters=3, lm_mu=1e-9))
@@ -49,8 +38,8 @@ def test_translation_only_reduces_to_the_data_term_solve(orc):
 
 def test_twist_explains_a_rotation_that_translations_cannot(orc):
     rng = np.random.default_rng(3)
-    node_pts, src = _patch(rng)
-    dst = src.copy(); dst[:, :3] = (src[:, :3] @ _rot_y(4.0).T + np.array([0.01, 0, 0.005])).astype(np.float32)
+    node_pts, src = node_patch(rng)
+    dst = src.copy(); dst[:, :3] = (src[:, :3] @ rot_y(4.0).T + np.array([0.01, 0, 0.005])).astype(np.float32)
     e = {}
     for flags in (0, orc.F2_TWIST):
         nodes = orc.make_nodes(node_pts, weight=0.08)
@@ -66,7 +55,7 @@ def test_twist_explains_a_rotation_that_translations_cannot(orc):
 
 def test_tukey_rejects_outliers_and_huber_regulariser_smooths(orc):
     rng = np.random.default_rng(9)
-    node_pts, src = _patch(rng)
+    node_pts, src = node_patch(rng)
     true_t = np.array([0.008, 0.0, -0.004], np.float32)
     dst = src.copy(); dst[:, :3] += true_t
     out = rng.choice(len(src), len(src) // 10, replace=False)

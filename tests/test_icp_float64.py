@@ -17,10 +17,6 @@ SCENE_CASES = [(s, v) for s in ic.SCENES for v in ic.scene_variants(s)]
 _SCENE_STEPS = {}
 
 
-def _acc_id(c):
-    return f"{c[0][0]}x{c[0][1]}-{c[1]}-{c[2]}"
-
-
 def test_launch_shape_reproduces_the_table():
     for (cols, rows), want in ic.LAUNCH_TABLE.items():
         assert ir.launch_shape(cols, rows) == want, (cols, rows)
@@ -28,7 +24,7 @@ def test_launch_shape_reproduces_the_table():
     assert ir.launch_shape(351, 288)[0] == 256 and ir.launch_shape(1, 1) == (256, 1, 1)
 
 
-@pytest.mark.parametrize("case", ACC_CASES, ids=_acc_id)
+@pytest.mark.parametrize("case", ACC_CASES, ids=ic.acc_id)
 def test_sums64_matches_oracle_accumulate(orc, case):
     (cols, rows), variant, pose = case
     curr, prev, Kl, T, dist2, min_cos = ic.accumulate_case(cols, rows, variant, pose)

@@ -17,11 +17,12 @@ import numpy as np
 import pytest
 
 torch = pytest.importorskip("torch")
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("orc")]
 
 import icp_cases as ic  # noqa: E402
 import icp_reference as ir  # noqa: E402
 from dynamicfusion_b200 import capi  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 SCRATCH = 32 + 27 * 1024                                   # DF_ICP_SCRATCH_DOUBLES
 SENTINEL = -1.2345e300
@@ -31,15 +32,6 @@ ACC_CASES = [(s, v, p) for s in ic.SIZES for v in ("points", "depth") for p in i
 SCENE_CASES = [(s, v) for s in ic.SCENES for v in ic.scene_variants(s)]
 _EST, _HOOK = {}, {}
 IDENTITY = (np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _oracle(orc):
-    return orc
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _dev(a, pad=0):
@@ -68,13 +60,9 @@ def _accumulate(variant, curr, prev, Kl, T, dist2, min_cos, padded=False):
     lib = capi.load()
     fn = lib.df_icp_accumulate if variant == "points" else lib.df_icp_accumulate_depth
     args = [x for t, p in maps for x in (t.data_ptr(), p)]
-    capi.check(fn(*args, cols, rows, capi.make_intr(*Kl), capi.make_aff(*T), float(dist2), float(min_cos), scratch.data_ptr(), _stream()))
+    capi.check(fn(*args, cols, rows, capi.make_intr(*Kl), capi.make_aff(*T), float(dist2), float(min_cos), scratch.data_ptr(), gu.stream()))
     torch.cuda.synchronize()
     return scratch.cpu().numpy()
-
-
-def _acc_id(c):
-    return f"{c[0][0]}x{c[0][1]}-{c[1]}-{c[2]}"
 
 
 def _check_table(scratch, blocks, finite=True):
@@ -89,7 +77,7 @@ def _check_table(scratch, blocks, finite=True):
     return table[:blocks]
 
 
-@pytest.mark.parametrize("case", ACC_CASES, ids=_acc_id)
+@pytest.mark.parametrize("case", ACC_CASES, ids=ic.acc_id)
 def test_accumulate_matches_float64_reference(case):
     (cols, rows), variant, pose = case
     curr, prev, Kl, T, dist2, min_cos = ic.accumulate_case(cols, rows, variant, pose)
@@ -176,12 +164,12 @@ def _estimate(variant, curr, prev, iters, levels=3, padded=False, K0=ic.K, scrat
         assert all(a[1] == b[1] == c[1] == d[1] for a, b, c, d in zip(vc, ncur, vp, npr))
         pitch = (C.c_size_t * L)(*[x[1] for x in vc])
         capi.check(lib.df_icp_estimate(arr(vc), arr(ncur), arr(vp), arr(npr), cols, rows, pitch, L, it, capi.make_intr(*K0), ic.DIST,
-                                       ic.ANGLE, Tdev.data_ptr(), okdev.data_ptr(), scratch.data_ptr(), _stream()))
+                                       ic.ANGLE, Tdev.data_ptr(), okdev.data_ptr(), scratch.data_ptr(), gu.stream()))
     else:
         dpitch = (C.c_size_t * L)(*[x[1] for x in vc])
         npitch = (C.c_size_t * L)(*[x[1] for x in ncur])
         capi.check(lib.df_icp_estimate_depth(arr(vc), arr(ncur), arr(vp), arr(npr), cols, rows, dpitch, npitch, L, it, capi.make_intr(*K0),
-                                             ic.DIST, ic.ANGLE, Tdev.data_ptr(), okdev.data_ptr(), scratch.data_ptr(), _stream()))
+                                             ic.DIST, ic.ANGLE, Tdev.data_ptr(), okdev.data_ptr(), scratch.data_ptr(), gu.stream()))
     torch.cuda.synchronize()
     T = Tdev.cpu().numpy()
     return (T[:9].reshape(3, 3).copy(), T[9:].copy()), int(okdev.item()), scratch.cpu().numpy()
@@ -259,7 +247,7 @@ def _hook_run(name, ok_in=1, offset=0):
     buf[offset:offset + 27 * n] = torch.from_numpy(table.reshape(-1)).cuda()
     Tdev = torch.from_numpy(np.concatenate([T_in[0].reshape(9), T_in[1]]).astype(np.float32)).cuda()
     okdev = torch.full((1,), ok_in, dtype=torch.int32, device="cuda")
-    status = capi.load().df_icp_solve_step(buf.data_ptr() + 8 * offset, n, Tdev.data_ptr(), okdev.data_ptr(), _stream())
+    status = capi.load().df_icp_solve_step(buf.data_ptr() + 8 * offset, n, Tdev.data_ptr(), okdev.data_ptr(), gu.stream())
     torch.cuda.synchronize()
     T = Tdev.cpu().numpy()
     return status, (T[:9].reshape(3, 3).copy(), T[9:].copy()), int(okdev.item()), sums, T_in

@@ -9,17 +9,9 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import capi, host, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 FRAMES = [synth.umbrella_depth(t) for t in range(5)]
-
-
-def _params(flags):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, 64, 1.0)
-    p.max_nodes = 512
-    p.cloud_capacity = 400000
-    p.flags = flags
-    return p
 
 
 # info()["launches"] after frames 0, 1 and 3 of synth.umbrella_depth at 64^3 (measured on an H100; host-side arithmetic, so they
@@ -31,7 +23,7 @@ LAUNCHES = {0: (16, 72, 72), kf.RIGID_ONLY: (14, 51, 51), kf.WARPED_INTEGRATE: (
 @pytest.mark.parametrize("timing", [0, kf.STAGE_TIMING], ids=["untimed", "timed"])
 @pytest.mark.parametrize("flags", list(LAUNCHES), ids=["default", "rigid_only", "warped_integrate", "extend_field", "use_depth", "f2_solve"])
 def test_launch_counts_and_stage_marks(flags, timing):
-    k = kf.KinFu(_params(flags | timing))
+    k = kf.KinFu(gu.kinfu_params(64, flags | timing, max_nodes=512, cloud_capacity=400000))
     launches, timed = [], []
     for t in range(4):
         k(FRAMES[t])
@@ -54,8 +46,8 @@ def _buffer_ptr(lib, k, name):
 
 def test_dynamicfusion_entry_equals_the_stage_inside_a_frame():
     lib = capi.load()
-    p = _params(0)
-    a, c = kf.KinFu(_params(0)), kf.KinFu(_params(0))
+    p = gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000)
+    a, c = (kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000)) for _ in range(2))
     for d in FRAMES[:4]:
         a(d)
         c(d)

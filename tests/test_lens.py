@@ -9,8 +9,7 @@ import pytest
 import color_camera_oracle as cco
 import lens_oracle as lo
 import snapshot_model as sm
-from test_color import _color_sections, _params, _v1_body, lib  # noqa: F401  (lib is a fixture)
-from test_color_camera import _camera_bytes
+from snapshot_model import lib  # noqa: F401  (a fixture)
 
 KV2_LENS = (0.09, -0.27, 0.0, 0.0, 0.09)                     # Kinect-v2-like barrel lens (k1, k2, p1, p2, k3)
 STRONG_LENS = (0.6, -0.1, 0.012, -0.009, 0.02, 0.2, -0.05, 0.01)   # eight-coefficient rational model with tangential terms
@@ -143,12 +142,12 @@ def test_snapshot_version_4_checks(lib):
     from dynamicfusion_b200 import capi
     from dynamicfusion_b200.kinfu import COLOR, KinFu
     assert C.sizeof(capi.Lens) == 36
-    p1, p2 = _params(capi, lib, 0), _params(capi, lib, COLOR)
+    p1, p2 = sm.small_params(capi, lib, 0), sm.small_params(capi, lib, COLOR)
     dims = tuple(p2.volume_dims)
-    v1 = _v1_body(capi, lib, p1)
-    length, cls, payload, rgba = _color_sections(dims)
-    v2 = _v1_body(capi, lib, p2) + length + cls + payload + rgba
-    cam = _camera_bytes(capi)
+    v1 = sm.v1_body(capi, lib, p1)
+    length, cls, payload, rgba = sm.color_sections(dims)
+    v2 = sm.v1_body(capi, lib, p2) + length + cls + payload + rgba
+    cam = sm.camera_bytes(capi)
     dl, cl = capi.make_lens(KV2_LENS, 1.0), capi.make_lens(STRONG_LENS, 1.5)
 
     def accepted(body, version=4):

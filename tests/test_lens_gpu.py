@@ -18,6 +18,7 @@ pytestmark = pytest.mark.gpu
 import color_camera_oracle as cco  # noqa: E402
 import lens_oracle as lo  # noqa: E402
 from dynamicfusion_b200 import build, capi, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 I3 = np.eye(3, dtype=np.float32)
@@ -26,28 +27,6 @@ STRONG_LENS = (0.6, -0.1, 0.012, -0.009, 0.02, 0.2, -0.05, 0.01)        # ration
 COLOR_LENS = (0.9, 0.25, 0.0, 0.0, 0.05)                                # a strong pincushion colour lens
 K_WIDE = (460.0, 460.0, 320.0, 240.0)                                   # 640 x 480 with a Kinect-v2-class field of view
 KV2_CAM = ((1081.37, 1081.37, 959.5, 539.5), 1920, 1080, (I3, np.array([-0.052, 0.0, 0.0], np.float32)))
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _dev(a):
-    a = np.ascontiguousarray(a)
-    view = {np.dtype(np.uint32): np.int32, np.dtype(np.uint16): np.int16}.get(a.dtype)
-    return torch.from_numpy(a.view(view) if view else a).cuda()
-
-
-def _host(t, dtype, shape):
-    return t.cpu().numpy().view(dtype).reshape(shape)
-
-
-def _padded(img, extra, fill):
-    """(device tensor with `extra` more elements per row, pitch in bytes, host view with the same strides)"""
-    rows, cols = img.shape[:2]
-    host = np.full((rows, cols + extra) + img.shape[2:], fill, img.dtype)
-    host[:, :cols] = img
-    return _dev(host), host.strides[0], host[:, :cols]
 
 
 def _lens(coeffs, K, cols, rows):
@@ -79,14 +58,14 @@ def test_undistort_equals_the_oracle(name, K, cols, rows, coeffs, pad):
     for with_bgra in (False, True):
         depth = synth.sphere_wall_depth(cols, rows, K, seed=1)
         bgra = rng.integers(0, 256, (rows, cols, 4), np.uint8)
-        d_dev, d_pitch, d_host = _padded(depth, pad, 7)
-        b_dev, b_pitch, b_host = _padded(bgra, pad, 9)
+        d_dev, d_pitch, d_host = gu.padded(depth, pad, 7)
+        b_dev, b_pitch, b_host = gu.padded(bgra, pad, 9)
         out = torch.full((rows, cols + pad + 1), 0x1234, dtype=torch.int16, device="cuda")
         bout = torch.full((rows, cols + pad + 2, 4), 77, dtype=torch.uint8, device="cuda")
         capi.check(lib.df_undistort(d_dev.data_ptr(), d_pitch, out.data_ptr(), (cols + pad + 1) * 2, b_dev.data_ptr() if with_bgra else None,
                                     b_pitch, bout.data_ptr() if with_bgra else None, (cols + pad + 2) * 4, cols, rows, capi.make_intr(*K), lens,
-                                    _stream()))
-        g = _host(out, np.uint16, (rows, cols + pad + 1))
+                                    gu.stream()))
+        g = gu.host(out, np.uint16, (rows, cols + pad + 1))
         gb = bout.cpu().numpy()
         want, want_b = lo.undistort(d_host, K, lens, b_host if with_bgra else None)
         assert np.array_equal(g[:, :cols], want), (name, with_bgra)
@@ -104,8 +83,8 @@ def test_undistort_equals_the_oracle(name, K, cols, rows, coeffs, pad):
 def test_undistort_refusals_write_nothing():
     lib = capi.load()
     K, cols, rows = synth.DEFAULT_K, 64, 48
-    depth = _dev(np.full((rows, cols), 1000, np.uint16))
-    bgra = _dev(np.full((rows, cols, 4), 5, np.uint8))
+    depth = gu.dev(np.full((rows, cols), 1000, np.uint16))
+    bgra = gu.dev(np.full((rows, cols, 4), 5, np.uint8))
     out = torch.full((rows, cols), 3, dtype=torch.int16, device="cuda")
     bout = torch.full((rows, cols, 4), 3, dtype=torch.uint8, device="cuda")
     good = _lens(KV2_LENS, K, cols, rows)
@@ -113,7 +92,7 @@ def test_undistort_refusals_write_nothing():
 
     def call(lens=good, dpitch=cols * 2, opitch=cols * 2, src=depth, dst=out, b=bgra, bo=bout, bpitch=cols * 4):
         return lib.df_undistort(src.data_ptr(), dpitch, dst.data_ptr(), opitch, None if b is None else b.data_ptr(), bpitch,
-                                None if bo is None else bo.data_ptr(), cols * 4, cols, rows, intr, lens, _stream())
+                                None if bo is None else bo.data_ptr(), cols * 4, cols, rows, intr, lens, gu.stream())
     assert call(lens=capi.make_lens((-0.5, 0, 0, 0, 0), 1.0)) != 0      # a folding lens
     assert call(lens=capi.make_lens(KV2_LENS, 0.0)) != 0                 # r2_max not > 0
     assert call(dpitch=cols * 2 - 2) != 0 and call(opitch=cols * 2 + 1) != 0 and call(bpitch=cols * 4 + 2) != 0
@@ -121,7 +100,7 @@ def test_undistort_refusals_write_nothing():
     assert call(bo=None) != 0                                            # bgra without its output
     assert call(bo=bgra) != 0                                            # colour in place
     torch.cuda.synchronize()
-    assert (out == 3).all() and (bout == 3).all() and (_host(depth, np.uint16, (rows, cols)) == 1000).all()
+    assert (out == 3).all() and (bout == 3).all() and (gu.host(depth, np.uint16, (rows, cols)) == 1000).all()
     assert call() == 0
 
 
@@ -158,37 +137,38 @@ def test_colour_kernels_equal_the_oracle(name, cols, rows, camera, coeffs, pad, 
     o_lens = np.zeros(nvox, np.uint32)
     for t in range(3):
         depth = synth.sphere_wall_depth(cols, rows, K, seed=t)
-        d_dev, d_pitch, d_host = _padded(depth, pad, 7)
+        d_dev, d_pitch, d_host = gu.padded(depth, pad, 7)
         dists = torch.zeros((rows, cols + pad), dtype=torch.int16, device="cuda")
-        capi.check(lib.df_compute_dists(d_dev.data_ptr(), d_pitch, cols, rows, intr, dists.data_ptr(), (cols + pad) * 2, _stream()))
+        capi.check(lib.df_compute_dists(d_dev.data_ptr(), d_pitch, cols, rows, intr, dists.data_ptr(), (cols + pad) * 2, gu.stream()))
         capi.check(lib.df_integrate_tracked(V, dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam), intr, None,
-                                            act.data_ptr(), None, _stream()))
+                                            act.data_ptr(), None, gu.stream()))
         maps = {}
         for key, lp in (("lens", C.byref(lens)), ("null", None), ("base", "base")):
             m = torch.full((mr, mc + cpad), 0x5a5a5a5a, dtype=torch.int32, device="cuda")
             if lp == "base":
-                capi.check(lib.df_color_depth_map(d_dev.data_ptr(), d_pitch, cols, rows, intr, cs, m.data_ptr(), (mc + cpad) * 4, _stream()))
+                capi.check(lib.df_color_depth_map(d_dev.data_ptr(), d_pitch, cols, rows, intr, cs, m.data_ptr(), (mc + cpad) * 4, gu.stream()))
             else:
-                capi.check(lib.df_color_depth_map_lens(d_dev.data_ptr(), d_pitch, cols, rows, intr, cs, lp, m.data_ptr(), (mc + cpad) * 4, _stream()))
+                capi.check(lib.df_color_depth_map_lens(d_dev.data_ptr(), d_pitch, cols, rows, intr, cs, lp, m.data_ptr(), (mc + cpad) * 4,
+                                                       gu.stream()))
             maps[key] = m
-        gmap = _host(maps["lens"], np.uint32, (mr, mc + cpad))
+        gmap = gu.host(maps["lens"], np.uint32, (mr, mc + cpad))
         assert np.all(gmap[:, mc:] == 0x5a5a5a5a)
         omap = lo.depth_map(d_host, K, cam, lens)
         assert np.array_equal(gmap[:, :mc], omap), (name, t)
-        assert np.array_equal(_host(maps["null"], np.uint32, (mr, mc + cpad)), _host(maps["base"], np.uint32, (mr, mc + cpad)))
+        assert np.array_equal(gu.host(maps["null"], np.uint32, (mr, mc + cpad)), gu.host(maps["base"], np.uint32, (mr, mc + cpad)))
         if name.endswith("zero"):
-            assert np.array_equal(gmap, _host(maps["base"], np.uint32, (mr, mc + cpad)))
+            assert np.array_equal(gmap, gu.host(maps["base"], np.uint32, (mr, mc + cpad)))
         img = rng.integers(0, 256, (cam.rows, cam.cols, 4), np.uint8)
-        i_dev, i_pitch, i_host = _padded(img, cpad, 99)
+        i_dev, i_pitch, i_host = gu.padded(img, cpad, 99)
         capi.check(lib.df_integrate_color_camera_lens(V, g_lens.data_ptr(), dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam),
                                                       intr, cs, C.byref(lens), i_dev.data_ptr(), i_pitch, maps["lens"].data_ptr(), (mc + cpad) * 4,
-                                                      act.data_ptr(), _stream()))
+                                                      act.data_ptr(), gu.stream()))
         capi.check(lib.df_integrate_color_camera_lens(V, g_null.data_ptr(), dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam),
                                                       intr, cs, None, i_dev.data_ptr(), i_pitch, maps["base"].data_ptr(), (mc + cpad) * 4,
-                                                      act.data_ptr(), _stream()))
+                                                      act.data_ptr(), gu.stream()))
         capi.check(lib.df_integrate_color_camera(V, g_base.data_ptr(), dists.data_ptr(), (cols + pad) * 2, cols, rows, capi.make_aff(*vol2cam),
                                                  intr, cs, i_dev.data_ptr(), i_pitch, maps["base"].data_ptr(), (mc + cpad) * 4, act.data_ptr(),
-                                                 _stream()))
+                                                 gu.stream()))
         assert np.array_equal(g_null.cpu().numpy(), g_base.cpu().numpy()), (name, t)   # a NULL lens is the entry without _lens
         dists_host = dists.cpu().numpy().view(np.uint16)[:, :cols]
         lo.integrate_color_camera(o_lens, dims, vs, trunc, 64, dists_host, vol2cam, K, cam, lens, i_host, omap, act.cpu().numpy())
@@ -196,21 +176,22 @@ def test_colour_kernels_equal_the_oracle(name, cols, rows, camera, coeffs, pad, 
         # frame intensity, level 0, from the frame's vertex map
         pts = torch.zeros((rows, cols, 4), dtype=torch.float32, device="cuda")
         nrm = torch.zeros_like(pts)
-        capi.check(lib.df_points_normals(intr, d_dev.data_ptr(), d_pitch, cols, rows, pts.data_ptr(), cols * 16, nrm.data_ptr(), cols * 16, _stream()))
+        capi.check(lib.df_points_normals(intr, d_dev.data_ptr(), d_pitch, cols, rows, pts.data_ptr(), cols * 16, nrm.data_ptr(), cols * 16,
+                                         gu.stream()))
         outs = {}
         for key, lp in (("lens", C.byref(lens)), ("null", None)):
             o = torch.full((rows, cols), 7.0, dtype=torch.float32, device="cuda")
             arr = lambda v, t_: (t_ * 1)(v)  # noqa: E731
             capi.check(lib.df_frame_intensity_lens(i_dev.data_ptr(), i_pitch, C.byref(cs), lp, intr, pts.data_ptr(), cols * 16,
                                                    maps[key if key == "lens" else "base"].data_ptr(), (mc + cpad) * 4, trunc, 1, arr(cols, C.c_int),
-                                                   arr(rows, C.c_int), arr(o.data_ptr(), C.c_void_p), arr(cols * 4, C.c_size_t), _stream()))
+                                                   arr(rows, C.c_int), arr(o.data_ptr(), C.c_void_p), arr(cols * 4, C.c_size_t), gu.stream()))
             outs[key] = o.cpu().numpy()
         base = torch.full((rows, cols), 7.0, dtype=torch.float32, device="cuda")
         capi.check(lib.df_frame_intensity(i_dev.data_ptr(), i_pitch, C.byref(cs), intr, pts.data_ptr(), cols * 16, maps["base"].data_ptr(),
                                           (mc + cpad) * 4, trunc, 1, (C.c_int * 1)(cols), (C.c_int * 1)(rows), (C.c_void_p * 1)(base.data_ptr()),
-                                          (C.c_size_t * 1)(cols * 4), _stream()))
+                                          (C.c_size_t * 1)(cols * 4), gu.stream()))
         want = lo.frame_intensity(i_host, K, cam, lens, omap, trunc, pts.cpu().numpy())
-        assert _same_or_nan(outs["lens"], want), (name, t)                 # the device's NaN has other payload bits than C's
+        assert gu.same_bits(outs["lens"], want), (name, t)                 # the device's NaN has other payload bits than C's
         assert np.array_equal(outs["null"].view(np.uint32), base.cpu().numpy().view(np.uint32))
         assert (~np.isnan(want)).mean() > 0.05
     w = g_lens.cpu().numpy().view(np.uint32) >> 24
@@ -221,10 +202,6 @@ def test_colour_kernels_equal_the_oracle(name, cols, rows, camera, coeffs, pad, 
         assert not np.array_equal(g_lens.cpu().numpy(), g_null.cpu().numpy())
 
 
-def _same_or_nan(a, b):
-    return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[~np.isnan(a)].view(np.uint32), b[~np.isnan(b)].view(np.uint32))
-
-
 def test_colour_kernels_refuse_an_invalid_lens():
     lib = capi.load()
     K, cols, rows = synth.DEFAULT_K, 64, 48
@@ -232,43 +209,28 @@ def test_colour_kernels_refuse_an_invalid_lens():
     cs = capi.make_color_camera(cam.K, cam.cols, cam.rows, cam.d2c)
     mc, mr, _ = cco.map_dims(K, cam)
     intr = capi.make_intr(*K)
-    depth = _dev(np.full((rows, cols), 1000, np.uint16))
+    depth = gu.dev(np.full((rows, cols), 1000, np.uint16))
     m = torch.full((mr, mc), 5, dtype=torch.int32, device="cuda")
     dims = (32, 32, 32)
     colours = torch.full((32 ** 3,), 9, dtype=torch.int32, device="cuda")
     V = capi.make_volume(colours.data_ptr(), dims, (3.0 / 32,) * 3, 0.2, 64)
-    dists = _dev(np.full((rows, cols), 0x3c00, np.uint16))                 # fp16 1.0 everywhere
-    img = _dev(np.full((cam.rows, cam.cols, 4), 200, np.uint8))
-    pts = _dev(np.tile(np.array([0.0, 0.0, 1.0, 1.0], np.float32), (rows, cols, 1)))
+    dists = gu.dev(np.full((rows, cols), 0x3c00, np.uint16))               # fp16 1.0 everywhere
+    img = gu.dev(np.full((cam.rows, cam.cols, 4), 200, np.uint8))
+    pts = gu.dev(np.tile(np.array([0.0, 0.0, 1.0, 1.0], np.float32), (rows, cols, 1)))
     inten = torch.full((rows, cols), 7.0, dtype=torch.float32, device="cuda")
     vol2cam = capi.make_aff(I3, np.array([-1.5, -1.5, 0.5], np.float32))
     for bad in (capi.make_lens((-0.5, 0, 0, 0, 0), 1.0), capi.make_lens((0,) * 5, 0.0), capi.make_lens((float("nan"), 0, 0, 0, 0), 1.0)):
-        assert lib.df_color_depth_map_lens(depth.data_ptr(), cols * 2, cols, rows, intr, cs, C.byref(bad), m.data_ptr(), mc * 4, _stream()) != 0
+        assert lib.df_color_depth_map_lens(depth.data_ptr(), cols * 2, cols, rows, intr, cs, C.byref(bad), m.data_ptr(), mc * 4, gu.stream()) != 0
         assert lib.df_integrate_color_camera_lens(V, colours.data_ptr(), dists.data_ptr(), cols * 2, cols, rows, vol2cam, intr, cs, C.byref(bad),
-                                                  img.data_ptr(), cam.cols * 4, m.data_ptr(), mc * 4, None, _stream()) != 0
+                                                  img.data_ptr(), cam.cols * 4, m.data_ptr(), mc * 4, None, gu.stream()) != 0
         assert lib.df_frame_intensity_lens(img.data_ptr(), cam.cols * 4, C.byref(cs), C.byref(bad), intr, pts.data_ptr(), cols * 16, m.data_ptr(),
                                            mc * 4, 0.2, 1, (C.c_int * 1)(cols), (C.c_int * 1)(rows), (C.c_void_p * 1)(inten.data_ptr()),
-                                           (C.c_size_t * 1)(cols * 4), _stream()) != 0
+                                           (C.c_size_t * 1)(cols * 4), gu.stream()) != 0
     torch.cuda.synchronize()
     assert (m == 5).all() and (colours == 9).all() and (inten == 7.0).all()
 
 
 # ----------------------------------------------------------------------------------------------------------------------- the frame loop
-def _params(dim=128, flags=0, K=None, cloud_capacity=1_000_000, size=1.0):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, size)
-    p.max_nodes = 1024
-    p.cloud_capacity = cloud_capacity
-    p.flags = flags
-    if K is not None:
-        p.intr.fx, p.intr.fy, p.intr.cx, p.intr.cy = K
-    return p
-
-
-def _state(k):
-    return k.state_digest(), [np.concatenate([a.reshape(-1) for a in k.getCameraPose(i)]).tobytes() for i in range(k.info()["poses"])]
-
-
 @functools.lru_cache(maxsize=None)
 def _lensed(t, camera=False):
     return synth.umbrella_rgbd(t, lens=KV2_LENS, color_camera=KV2_CAM + (COLOR_LENS,) if camera else None)
@@ -276,7 +238,7 @@ def _lensed(t, camera=False):
 
 @pytest.mark.parametrize("flags,camera", [(0, False), (kf.COLOR, True)], ids=["default", "color_camera"])
 def test_zero_lens_is_no_lens(flags, camera):
-    objs = [kf.KinFu(_params(flags=flags)) for _ in range(2)]
+    objs = [kf.KinFu(gu.kinfu_params(128, flags, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2)]
     zero = (0.0,) * 8
     if camera:
         objs[0].set_color_camera(*KV2_CAM)
@@ -287,7 +249,7 @@ def test_zero_lens_is_no_lens(flags, camera):
         depth, bgra = synth.umbrella_rgbd(t, color_camera=KV2_CAM if camera else None)
         for k in objs:
             k(depth, bgra) if flags & kf.COLOR else k(depth)
-        assert _state(objs[0]) == _state(objs[1]) and objs[0].info() == objs[1].info()
+        assert gu.state(objs[0]) == gu.state(objs[1]) and objs[0].info() == objs[1].info()
         if camera:
             assert np.array_equal(objs[0].buffer("color_volume"), objs[1].buffer("color_volume"))
     assert objs[0].snapshot() == objs[1].snapshot()                     # a zero lens writes no version-4 section
@@ -298,14 +260,14 @@ def test_zero_lens_is_no_lens(flags, camera):
 def _undistort_on_device(k, depth, bgra):
     """the frame as the object with a depth lens sees it, from df_undistort: device (depth, bgra or None)"""
     p = k.params
-    d, out = _dev(depth), torch.zeros((p.rows, p.cols), dtype=torch.int16, device="cuda")
+    d, out = gu.dev(depth), torch.zeros((p.rows, p.cols), dtype=torch.int16, device="cuda")
     b = bout = None
     if bgra is not None and bgra.shape[:2] == depth.shape:
-        b, bout = _dev(bgra), torch.zeros((p.rows, p.cols, 4), dtype=torch.uint8, device="cuda")
+        b, bout = gu.dev(bgra), torch.zeros((p.rows, p.cols, 4), dtype=torch.uint8, device="cuda")
     capi.check(k.lib.df_undistort(d.data_ptr(), p.cols * 2, out.data_ptr(), p.cols * 2, None if b is None else b.data_ptr(), p.cols * 4,
-                                  None if bout is None else bout.data_ptr(), p.cols * 4, p.cols, p.rows, p.intr, k.depth_lens, _stream()))
+                                  None if bout is None else bout.data_ptr(), p.cols * 4, p.cols, p.rows, p.intr, k.depth_lens, gu.stream()))
     torch.cuda.synchronize()
-    return out, (bout if bout is not None else (None if bgra is None else _dev(bgra)))
+    return out, (bout if bout is not None else (None if bgra is None else gu.dev(bgra)))
 
 
 @pytest.mark.parametrize("overlap", ["1", "0"])
@@ -313,17 +275,17 @@ def _undistort_on_device(k, depth, bgra):
 def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap, camera):
     """an object with a depth lens fed raw frames equals one without, fed df_undistort's output of the same frames"""
     monkeypatch.setenv("DF_KINFU_OVERLAP_EXTRACT", overlap)
-    lensed, plain = kf.KinFu(_params(flags=kf.COLOR)), kf.KinFu(_params(flags=kf.COLOR))
+    lensed, plain = (kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2))
     lensed.set_depth_lens(KV2_LENS)
     if camera:
         for k in (lensed, plain):
             k.set_color_camera(*KV2_CAM, lens=COLOR_LENS)
     for t in range(6):
         depth, bgra = _lensed(t, camera)
-        lensed(_dev(depth), _dev(bgra))                                  # device frames: the caller's buffers are never written
+        lensed(gu.dev(depth), gu.dev(bgra))                              # device frames: the caller's buffers are never written
         d, b = _undistort_on_device(lensed, depth, bgra)
         plain(d, b)
-        assert _state(lensed) == _state(plain)
+        assert gu.state(lensed) == gu.state(plain)
         assert lensed.info()["launches"] == plain.info()["launches"] + 1
         assert np.array_equal(lensed.buffer("color_volume"), plain.buffer("color_volume"))
         assert np.array_equal(lensed.buffer("cloud_colors"), plain.buffer("cloud_colors"))
@@ -336,18 +298,18 @@ def test_loop_rebuilt_from_the_public_entries(monkeypatch, overlap, camera):
 
 
 def test_caller_frames_are_not_written():
-    k = kf.KinFu(_params(flags=kf.COLOR))
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     k.set_depth_lens(KV2_LENS)
     depth, bgra = _lensed(0)
-    d, b = _dev(depth), _dev(bgra)
+    d, b = gu.dev(depth), gu.dev(bgra)
     k(d, b)
     torch.cuda.synchronize()
-    assert np.array_equal(_host(d, np.uint16, depth.shape), depth) and np.array_equal(b.cpu().numpy(), bgra)
+    assert np.array_equal(gu.host(d, np.uint16, depth.shape), depth) and np.array_equal(b.cpu().numpy(), bgra)
     k.close()
 
 
 def test_setters_follow_the_colour_camera_rules():
-    k = kf.KinFu(_params(flags=kf.COLOR))
+    k = kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
     with pytest.raises(RuntimeError):
         k.set_depth_lens(capi.make_lens((-0.5, 0, 0, 0, 0), 1.0))      # invalid: nothing changes
     assert k.depth_lens is None
@@ -369,7 +331,7 @@ def test_setters_follow_the_colour_camera_rules():
     k.set_depth_lens(None)
     k.set_color_camera(*KV2_CAM[:3], KV2_CAM[3])                         # a new camera drops the colour lens
     assert k.color_lens is None
-    plain = kf.KinFu(_params(flags=0))
+    plain = kf.KinFu(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000))
     plain.set_depth_lens(KV2_LENS)                                       # a depth lens on any object
     plain(_lensed(0)[0])
     assert plain.info()["frame_counter"] == 1
@@ -380,7 +342,7 @@ def test_setters_follow_the_colour_camera_rules():
 def test_registered_images_after_a_camera_is_removed(lens_first):
     """the registered image's buffer follows the camera: a depth lens set before or after a colour camera, then the camera removed, undistorts
     registered images as an object that never had a camera does"""
-    k, ref = kf.KinFu(_params(flags=kf.COLOR)), kf.KinFu(_params(flags=kf.COLOR))
+    k, ref = (kf.KinFu(gu.kinfu_params(128, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2))
     ref.set_depth_lens(KV2_LENS)
     if lens_first:
         k.set_depth_lens(KV2_LENS)
@@ -395,7 +357,7 @@ def test_registered_images_after_a_camera_is_removed(lens_first):
         depth, bgra = _lensed(t)
         k(depth, bgra)
         ref(depth, bgra)
-        assert _state(k) == _state(ref) and k.info()["launches"] == ref.info()["launches"]
+        assert gu.state(k) == gu.state(ref) and k.info()["launches"] == ref.info()["launches"]
         assert np.array_equal(k.buffer("color_volume"), ref.buffer("color_volume"))
     k.close(); ref.close()
 
@@ -404,7 +366,7 @@ def test_registered_images_after_a_camera_is_removed(lens_first):
                                    kf.WARPED_INTEGRATE],
                          ids=["live_model", "color_tracking", "use_depth", "extend_field", "f2_solve", "warped_integrate"])
 def test_flags_run_with_a_depth_lens(flags):
-    k = kf.KinFu(_params(flags=flags))
+    k = kf.KinFu(gu.kinfu_params(128, flags, max_nodes=1024, cloud_capacity=1_000_000))
     k.set_depth_lens(KV2_LENS)
     for t in range(5):
         depth, bgra = _lensed(t)
@@ -447,7 +409,7 @@ def test_tracking_fidelity_rigid_c2_256():
     n = 20
     runs, frame0 = {}, {}
     for name, lens_frames, lens_set in (("pinhole", None, False), ("lens", KV2_LENS, True), ("lens_ignored", KV2_LENS, False)):
-        k = kf.KinFu(_params(dim=256, flags=kf.RIGID_ONLY, K=K_WIDE, cloud_capacity=2_000_000, size=3.0))
+        k = kf.KinFu(gu.kinfu_params(256, kf.RIGID_ONLY, max_nodes=1024, cloud_capacity=2_000_000, size=3.0, K=K_WIDE))
         if lens_set:
             k.set_depth_lens(KV2_LENS)
         for t in range(n):
@@ -501,7 +463,7 @@ def test_texture_fidelity_through_a_lensed_colour_camera():
     stats = {}
     frames = [synth.umbrella_rgbd(t, color_camera=KV2_CAM + (COLOR_LENS,)) for t in range(20)]
     for name, lens in (("lens", COLOR_LENS), ("lens_ignored", None)):
-        k = kf.KinFu(_params(dim=256, flags=kf.COLOR, cloud_capacity=2_000_000))
+        k = kf.KinFu(gu.kinfu_params(256, kf.COLOR, max_nodes=1024, cloud_capacity=2_000_000))
         k.set_color_camera(*KV2_CAM, lens=lens)
         for f in frames:
             k(*f)
@@ -529,7 +491,7 @@ def test_version_4_resumes_and_rejects(tmp_path, capfd):
     frames = [_lensed(t, True) for t in range(7)]
 
     def make(depth_lens=KV2_LENS, color_lens=COLOR_LENS):
-        k = kf.KinFu(_params(dim=64, flags=kf.COLOR))
+        k = kf.KinFu(gu.kinfu_params(64, kf.COLOR, max_nodes=1024, cloud_capacity=1_000_000))
         k.set_color_camera(*KV2_CAM, lens=color_lens)
         if depth_lens is not None:
             k.set_depth_lens(depth_lens)

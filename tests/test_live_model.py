@@ -10,10 +10,10 @@ import numpy as np
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 
+import color_oracle  # noqa: E402
 import correspond_oracle as co  # noqa: E402
 import raster_oracle  # noqa: E402
-from test_mesh import IDENT  # noqa: E402
-from test_raster import K_EXACT, SPHERE_COLS, SPHERE_K, SPHERE_ROWS, _plane_verts, look_at, sphere_mesh  # noqa: E402
+from scenes import IDENT, K_EXACT, SPHERE_COLS, SPHERE_K, SPHERE_ROWS, look_at, plane_verts, sphere_mesh  # noqa: E402
 
 
 def _rot(ax, ay, az):
@@ -31,7 +31,7 @@ def _moved(verts, R, t):
 
 
 def _quad():
-    verts = _plane_verts([(2, 2), (10, 2), (10, 8), (2, 8)])
+    verts = plane_verts([(2, 2), (10, 2), (10, 8), (2, 8)])
     return verts, np.array([[0, 2, 1], [0, 3, 2]], np.int32), IDENT, K_EXACT, 16, 12
 
 
@@ -149,8 +149,7 @@ def test_no_correspondence_cases_write_nans():
 def test_host_affine_helpers_match_numpy():
     A = (_rot(0.1, 0.2, -0.3).astype(np.float32), np.array([0.1, -0.2, 0.3], np.float32))
     B = (_rot(-0.2, 0.05, 0.4).astype(np.float32), np.array([-0.05, 0.02, 0.7], np.float32))
-    R, t = co.aff_mul(A, B)
+    R, t = color_oracle.aff_mul(A, B)
     assert np.allclose(R, A[0].astype(np.float64) @ B[0], atol=1e-6) and np.allclose(t, A[0].astype(np.float64) @ B[1] + A[1], atol=1e-6)
-    Ri, ti = co.aff_inv(A)
+    Ri, ti = color_oracle.aff_inv(A)
     assert np.allclose(Ri @ A[0], np.eye(3), atol=1e-6) and np.allclose(Ri @ A[1] + ti, 0, atol=1e-6)
-    assert raster_oracle.aff_inv(*A)[0].tobytes() == Ri.tobytes()

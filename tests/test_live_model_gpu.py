@@ -14,23 +14,15 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import capi, kinfu as kf, synth  # noqa: E402
+import color_oracle  # noqa: E402
 import correspond_oracle as co  # noqa: E402
+import gpu_util as gu  # noqa: E402
 import raster_oracle  # noqa: E402
-from test_raster import look_at, sphere_mesh  # noqa: E402
-from test_raster_gpu import K640, _erode, _gpu_raster  # noqa: E402
+from scenes import K640, look_at, sphere_mesh  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 FRAMES = [synth.umbrella_depth(t) for t in range(15)]
 IDENT = (np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
-
-
-def _params(dim=128, flags=kf.LIVE_MODEL, cloud_capacity=1_000_000):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = 1024
-    p.cloud_capacity = cloud_capacity
-    p.flags = flags
-    return p
 
 
 def _t(a, dtype=torch.float32):
@@ -81,7 +73,7 @@ def test_correspond_equals_the_oracle():
              ("close_up", look_at(centre, 0.24, (-0.1, 0.15, 1.0)), K640, 640, 480),
              ("ragged", look_at(centre, 0.6, (0.2, 0.1, 1.0)), (180.0, 170.0, 61.3, 97.8), 203, 151)]
     for name, w2c, K, cols, rows in cases:
-        ids, pts, _, stats = _gpu_raster(cloud, tris, w2c, K, cols, rows)
+        ids, pts, _, stats = gu.gpu_raster(cloud, tris, w2c, K, cols, rows)
         if name == "close_up":
             assert stats[3] > 0                                          # the large-triangle path drew some of these pixels
         drawn = ids >= 0
@@ -98,7 +90,7 @@ def test_correspond_equals_the_oracle():
                     assert 0 < (drawn & ~kept).sum() < drawn.sum() // 2          # the distance test removes some pixels, not most
     # xyz rows (vstride 3)
     w2c = look_at(centre, 0.5, (0.3, -0.2, 1.0))
-    ids, pts, _, _ = _gpu_raster(cloud, tris, w2c, K640, 640, 480)
+    ids, pts, _, _ = gu.gpu_raster(cloud, tris, w2c, K640, 640, 480)
     want = co.correspond(ids, pts, cloud[:, :3], src[:, :3], tris, w2c)
     got = _gpu_correspond(ids, pts, cloud[:, :3], src[:, :3], tris, w2c)
     assert _same_bits(got[0], want[0]) and _same_bits(got[1], want[1])
@@ -160,16 +152,16 @@ def _K(p):
 
 
 def test_icp_reference_is_the_rendered_live_model():
-    k = kf.KinFu(_params(dim=256))
+    k = kf.KinFu(gu.kinfu_params(256, kf.LIVE_MODEL, max_nodes=1024, cloud_capacity=1_000_000))
     p = k.params
-    ident_w2c = co.aff_inv(IDENT)                                        # dfh_aff_inv of the identity, as the loop forms it
+    ident_w2c = color_oracle.aff_inv(IDENT)                              # dfh_aff_inv of the identity, as the loop forms it
     checked = 0
     for t, d in enumerate(FRAMES[:12]):
         fused = k(d)
         if not fused or k.info()["nodes"] < 8:
             continue
         _, live, faces = _live_mesh(k)
-        ids, pts, nrm, _ = _gpu_raster(live, faces, ident_w2c, _K(p), p.cols, p.rows)
+        ids, pts, nrm, _ = gu.gpu_raster(live, faces, ident_w2c, _K(p), p.cols, p.rows)
         assert _same_bits(k.buffer("prev_points"), pts), t
         assert _same_bits(k.buffer("prev_normals"), nrm), t
         assert (ids >= 0).sum() > 50000, t
@@ -179,7 +171,7 @@ def test_icp_reference_is_the_rendered_live_model():
 
 
 def test_association_is_the_correspondence_on_the_kept_live_mesh():
-    k = kf.KinFu(_params(dim=256))
+    k = kf.KinFu(gu.kinfu_params(256, kf.LIVE_MODEL, max_nodes=1024, cloud_capacity=1_000_000))
     p = k.params
     checked = 0
     for t in range(8):
@@ -191,9 +183,9 @@ def test_association_is_the_correspondence_on_the_kept_live_mesh():
         nxt = synth.compose(pose_t, (synth.camera_drift(1)[0].astype(np.float32), np.array([0.002, -0.001, 0.0005], np.float32)))
         k.set_overrides(pose=nxt)
         assert k(FRAMES[t + 1])
-        cam2model = co.aff_mul(co.aff_inv(pose_t), nxt)
-        w2c = co.aff_inv(cam2model)
-        ids, pts, _, _ = _gpu_raster(live, faces, w2c, _K(p), p.cols, p.rows)
+        cam2model = color_oracle.aff_mul(color_oracle.aff_inv(pose_t), nxt)
+        w2c = color_oracle.aff_inv(cam2model)
+        ids, pts, _, _ = gu.gpu_raster(live, faces, w2c, _K(p), p.cols, p.rows)
         want = _gpu_correspond(ids, pts, live, src, faces, w2c, k.buffer("curr_points"), p.icp_dist_thres)
         assert _same_bits(k.buffer("canonical_visible"), want[0]), t
         assert (~np.isnan(want[0][..., 0])).sum() > 50000
@@ -210,7 +202,7 @@ def _state(k):
 
 @pytest.mark.parametrize("extra", [0, kf.WARPED_INTEGRATE | kf.EXTEND_FIELD])
 def test_two_objects_agree_after_every_frame(extra):
-    a, b = kf.KinFu(_params(flags=kf.LIVE_MODEL | extra)), kf.KinFu(_params(flags=kf.LIVE_MODEL | extra))
+    a, b = (kf.KinFu(gu.kinfu_params(128, kf.LIVE_MODEL | extra, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2))
     for t, d in enumerate(FRAMES):
         assert a(d) == b(d)
         assert _state(a) == _state(b), t
@@ -220,7 +212,7 @@ def test_two_objects_agree_after_every_frame(extra):
 
 
 def test_resume_equals_the_uninterrupted_run(tmp_path):
-    ref = kf.KinFu(_params())
+    ref = kf.KinFu(gu.kinfu_params(128, kf.LIVE_MODEL, max_nodes=1024, cloud_capacity=1_000_000))
     states = []
     snaps = {}
     for t, d in enumerate(FRAMES[:12]):
@@ -230,7 +222,7 @@ def test_resume_equals_the_uninterrupted_run(tmp_path):
             snaps[t] = ref.snapshot()
     ref.close()
     for t0, data in snaps.items():
-        k = kf.KinFu(_params())
+        k = kf.KinFu(gu.kinfu_params(128, kf.LIVE_MODEL, max_nodes=1024, cloud_capacity=1_000_000))
         k.restore(data)
         for t in range(t0 + 1, 12):
             k(FRAMES[t])
@@ -239,7 +231,7 @@ def test_resume_equals_the_uninterrupted_run(tmp_path):
 
 
 def test_mesh_and_render_between_frames_change_nothing():
-    a, b = kf.KinFu(_params()), kf.KinFu(_params())
+    a, b = (kf.KinFu(gu.kinfu_params(128, kf.LIVE_MODEL, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2))
     for t, d in enumerate(FRAMES[:10]):
         a(d)
         b(d)
@@ -255,8 +247,8 @@ def test_mesh_and_render_between_frames_change_nothing():
     b.close()
 
 
-def _digests(flags, frames, **kw):
-    k = kf.KinFu(_params(flags=flags, **kw))
+def _digests(flags, frames, cloud_capacity=1_000_000):
+    k = kf.KinFu(gu.kinfu_params(128, flags, max_nodes=1024, cloud_capacity=cloud_capacity))
     out = []
     for d in frames:
         k(d)
@@ -297,7 +289,7 @@ def test_static_scene_stays_put():
     # 0.5159 deg, hit-mask agreement 0.9988, |dz| median 0.3102 voxel, p99 1.1120.  They are set about 1.5 times above it.  The pose drifts
     # on a scene that does not move, which is worth knowing: the translation-only data term has no regulariser, so the warp field can take
     # up a rigid offset as readily as the camera pose can.
-    k = kf.KinFu(_params(dim=256))
+    k = kf.KinFu(gu.kinfu_params(256, kf.LIVE_MODEL, max_nodes=1024, cloud_capacity=1_000_000))
     p = k.params
     frames = [synth.umbrella_depth(t, drift=False, shape_t=0) for t in range(10)]
     for d in frames:
@@ -319,8 +311,8 @@ def test_static_scene_stays_put():
     V = capi.make_volume(ptr.value, p.volume_dims, [p.volume_size[d] / p.volume_dims[d] for d in range(3)], max(p.tsdf_trunc_dist, 2.1 * vs),
                          p.tsdf_max_weight)
     vol_pose = (np.array(list(p.volume_pose.R), np.float32).reshape(3, 3), np.array(list(p.volume_pose.t), np.float32))
-    cam2vol = co.aff_mul(co.aff_inv(vol_pose), k.getCameraPose())
-    Rinv = co.aff_inv((cam2vol[0], np.zeros(3, np.float32)))[0]
+    cam2vol = color_oracle.aff_mul(color_oracle.aff_inv(vol_pose), k.getCameraPose())
+    Rinv = color_oracle.aff_inv((cam2vol[0], np.zeros(3, np.float32)))[0]
     rc = torch.empty((p.rows, p.cols, 4), device="cuda")
     rn = torch.empty_like(rc)
     capi.check(lib.df_raycast_points(V, capi.make_aff(*cam2vol), capi.f9(Rinv), p.intr, p.cols, p.rows, p.raycast_step_factor,
@@ -329,9 +321,9 @@ def test_static_scene_stays_put():
     pts = k.buffer("prev_points")
     k.close()
     hit_r, hit_m = ~np.isnan(rc[..., 2]), ~np.isnan(pts[..., 2])
-    uniform = (_erode(hit_r) | _erode(~hit_r)) & (_erode(hit_m) | _erode(~hit_m))
+    uniform = (gu.erode(hit_r) | gu.erode(~hit_r)) & (gu.erode(hit_m) | gu.erode(~hit_m))
     agree = (hit_r == hit_m)[uniform].mean()
-    both = _erode(hit_r) & _erode(hit_m)
+    both = gu.erode(hit_r) & gu.erode(hit_m)
     ray = rc[..., :3] / np.linalg.norm(rc[..., :3], axis=-1, keepdims=True)
     cosine = -np.einsum("ijk,ijk->ij", np.nan_to_num(rn[..., :3]), np.nan_to_num(ray))
     sel = both & (cosine > 0.3)

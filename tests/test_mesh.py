@@ -15,6 +15,7 @@ sys.path.insert(0, str(ROOT))
 
 import mesh_oracle  # noqa: E402
 from oracle import orc  # noqa: E402
+from scenes import IDENT, pack, sphere_volume  # noqa: E402
 
 CORNERS = np.array([[0, 0, 0], [1, 0, 0], [1, 1, 0], [0, 1, 0], [0, 0, 1], [1, 0, 1], [1, 1, 1], [0, 1, 1]])
 EDGES = [(0, 1), (1, 2), (3, 2), (0, 3), (4, 5), (5, 6), (7, 6), (4, 7), (0, 4), (1, 5), (2, 6), (3, 7)]
@@ -110,22 +111,6 @@ def test_winding_faces_free_space():
 
 
 # ------------------------------------------------------------------ oracle on analytic volumes --------------------------------------------
-IDENT = (np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
-
-
-def pack(F, W=1):
-    return (np.asarray(F, np.float16).view(np.uint16).astype(np.uint32) | (np.uint32(W) << np.uint32(16))).ravel()
-
-
-def sphere_volume(dims=(64, 60, 56), vs=0.01, radius_vox=20.3, centre_vox=(31.6, 29.8, 27.3), trunc_vox=4.0):
-    Dx, Dy, Dz = dims
-    z, y, x = np.meshgrid(np.arange(Dz), np.arange(Dy), np.arange(Dx), indexing="ij")
-    c = np.asarray(centre_vox) * vs
-    d = np.sqrt(((x + 0.5) * vs - c[0]) ** 2 + ((y + 0.5) * vs - c[1]) ** 2 + ((z + 0.5) * vs - c[2]) ** 2) - radius_vox * vs
-    F = np.clip(d / (trunc_vox * vs), -1.0, 1.0)
-    return pack(F), dims, (vs, vs, vs), trunc_vox * vs, c, radius_vox * vs
-
-
 def mesh_of(vol, dims, vsz, trunc):
     cloud = orc.extract_cloud(vol, dims, vsz, trunc, 64, IDENT, int(np.prod(dims)) * 3)
     tris = mesh_oracle.mesh(vol, dims, len(cloud))

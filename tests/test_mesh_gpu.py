@@ -13,9 +13,10 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import capi, host, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 import mesh_oracle  # noqa: E402
 from oracle import orc  # noqa: E402
-from test_mesh import pack, sphere_volume  # noqa: E402
+from scenes import pack, sphere_volume  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 IDENT = (np.eye(3, dtype=np.float32), np.zeros(3, np.float32))
@@ -67,23 +68,10 @@ def _gpu_mesh(vol_np, dims, vs, trunc, use_activity):
     return cloud[:n].cpu().numpy(), out[:T]
 
 
-def _c1_volume():
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, 256, 1.0)
-    p.flags = kf.RIGID_ONLY
-    p.cloud_capacity = 2_000_000
-    k = kf.KinFu(p)
-    for t in range(3):
-        k(synth.umbrella_depth(t))
-    vol = k.buffer("volume").copy()
-    k.close()
-    return vol, (256, 256, 256), 1.0 / 256, 0.04
-
-
 def _cases():
     sph = sphere_volume()
     yield "sphere", sph[0], sph[1], sph[2][0], sph[3]
-    yield ("c1_256",) + _c1_volume()
+    yield ("c1_256",) + gu.c1_volume()
     odd = sphere_volume(dims=(99, 70, 45), radius_vox=17.2, centre_vox=(50.3, 33.1, 22.6))
     yield "odd_99x70x45", odd[0], odd[1], odd[2][0], odd[3]
     big = sphere_volume(dims=(256, 256, 80), radius_vox=30.4, centre_vox=(120.2, 131.7, 40.3))
@@ -120,27 +108,11 @@ def test_plane_mesh_on_the_gpu():
 
 
 # ------------------------------------------------------------------ the frame loop ------------------------------------------------------------
-def _params(dim=128, flags=0, cloud_capacity=1_000_000):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = 1024
-    p.cloud_capacity = cloud_capacity
-    p.flags = flags
-    return p
-
-
 FRAMES = [synth.umbrella_depth(t) for t in range(10)]
 
 
-def _run(frames, **kw):
-    k = kf.KinFu(_params(**kw))
-    for d in frames:
-        k(d)
-    return k
-
-
 def test_vertices_are_the_cloud_and_state_is_unchanged():
-    k = _run(FRAMES[:6])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:6])
     before = k.state_digest()
     v, n, f = k.mesh()
     assert k.state_digest() == before
@@ -156,7 +128,7 @@ def test_vertices_are_the_cloud_and_state_is_unchanged():
 @pytest.mark.parametrize("overlap", ["1", "0"])
 def test_meshing_every_frame_changes_nothing(monkeypatch, overlap):
     monkeypatch.setenv("DF_KINFU_OVERLAP_EXTRACT", overlap)
-    a, b = kf.KinFu(_params()), kf.KinFu(_params())
+    a, b = (kf.KinFu(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2))
     for t, d in enumerate(FRAMES[:8]):
         a(d)
         b(d)
@@ -169,7 +141,7 @@ def test_meshing_every_frame_changes_nothing(monkeypatch, overlap):
 
 
 def test_sequence_mesh_is_a_consistently_wound_manifold():
-    k = _run(FRAMES)
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES)
     _, _, f = k.mesh()
     k.close()
     und = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), 1)
@@ -181,7 +153,7 @@ def test_sequence_mesh_is_a_consistently_wound_manifold():
 
 
 def test_live_mesh_is_the_loops_warp_of_the_cloud():
-    k = _run(FRAMES[:6])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:6])
     assert k.info()["nodes"] >= 8
     vc, nc, fc = k.mesh()
     vl, nl, fl = k.mesh(live=True)
@@ -205,7 +177,7 @@ def test_live_mesh_is_the_loops_warp_of_the_cloud():
 
 
 def test_live_mesh_needs_a_warp_field():
-    k = _run(FRAMES[:3], flags=kf.RIGID_ONLY)
+    k = gu.run(gu.kinfu_params(128, kf.RIGID_ONLY, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:3])
     assert k.info()["nodes"] < 8
     with pytest.raises(RuntimeError):
         k.mesh(live=True)
@@ -214,14 +186,14 @@ def test_live_mesh_needs_a_warp_field():
 
 def test_failures_write_nothing():
     lib = capi.load()
-    k = _run(FRAMES[:4], cloud_capacity=2000)                              # the cloud is cut at 2000 points
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=2000), FRAMES[:4])  # the cloud is cut at 2000 points
     assert k.info()["cloud_points"] == 2000
     before = k.state_digest()
     with pytest.raises(RuntimeError):
         k.mesh()
     assert k.state_digest() == before
     k.close()
-    k = _run(FRAMES[:4])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:4])
     nv, nt = C.c_int(), C.c_int()
     capi.check(lib.df_kinfu_mesh(k.h, 0, None, None, None, 0, 0, C.byref(nv), C.byref(nt)))
     v = np.full((nv.value, 3), 7.0, np.float32)
@@ -234,7 +206,7 @@ def test_failures_write_nothing():
 
 
 def test_restored_object_gives_the_same_mesh(tmp_path):
-    k = _run(FRAMES[:6])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:6])
     want = [k.mesh(), k.mesh(live=True)]
     k.save(tmp_path / "s.dfsnap")
     k.close()

@@ -19,20 +19,12 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import kinfu as kf, synth  # noqa: E402
-
-
-def _params(dim, max_nodes, flags=0):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = max_nodes
-    p.cloud_capacity = 1_000_000 if dim <= 128 else 4_000_000
-    p.flags = flags
-    return p
+import gpu_util as gu  # noqa: E402
 
 
 def _lockstep(orc, frames, dim, max_nodes, inject_nodes):
     from oracle import orc_pipe
-    p = _params(dim, max_nodes)
+    p = gu.kinfu_params(dim, 0, max_nodes=max_nodes, cloud_capacity=1_000_000 if dim <= 128 else 4_000_000)
     gpu, cpu = kf.KinFu(p), orc_pipe.KinFu(orc_pipe.params_from(p))
     diffs = []
     for t in range(frames):
@@ -82,7 +74,7 @@ def test_long_sequence_lockstep_50_frames(orc):
     BVH, row assembly, the LM/PCG solve with 120-240 iterations, both warps, project-and-remove, integrate, extraction -- runs on
     its own for 50 frames and is compared frame by frame."""
     from oracle import orc_pipe
-    p = _params(128, 2048)
+    p = gu.kinfu_params(128, 0, max_nodes=2048, cloud_capacity=1_000_000)
     p.node_step = 8                                       # ~1.9k nodes on the 128^3 cloud: the bench's node count
     gpu, cpu = kf.KinFu(p), orc_pipe.KinFu(orc_pipe.params_from(p))
     F = 50
@@ -121,7 +113,7 @@ def test_long_sequence_lockstep_50_frames(orc):
 def test_c2_three_frames(orc):
     """BASELINE configs[1] = the bench line's own configuration: 512^3 / 1 m, 2,036 nodes, three frames against the oracle's loop"""
     from oracle import orc_pipe
-    p = _params(512, 2048)
+    p = gu.kinfu_params(512, 0, max_nodes=2048, cloud_capacity=4_000_000)
     gpu, cpu = kf.KinFu(p), orc_pipe.KinFu(orc_pipe.params_from(p))
     for t in range(3):
         d = synth.umbrella_depth(t)

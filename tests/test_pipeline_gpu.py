@@ -12,25 +12,13 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import kinfu as kf, synth  # noqa: E402
-
-
-def _params(dim, flags=0, max_nodes=512):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = max_nodes
-    p.cloud_capacity = 400000
-    p.flags = flags
-    return p
-
-
-def _tsdf(vol):
-    return (vol & 0xffff).astype(np.uint16).view(np.float16).astype(np.float32), vol >> 16
+import gpu_util as gu  # noqa: E402
 
 
 @pytest.mark.parametrize("flags", [0, kf.RIGID_ONLY])
 def test_sequence_matches_oracle(orc, flags):
     from oracle import orc_pipe
-    p = _params(64, flags)
+    p = gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000)
     gpu = kf.KinFu(p)
     cpu = orc_pipe.KinFu(orc_pipe.params_from(p))
     frames = [synth.umbrella_depth(t) for t in range(4)]
@@ -46,8 +34,8 @@ def test_sequence_matches_oracle(orc, flags):
         Rc, tc = cpu.getCameraPose(t)
         assert np.abs(Rg - Rc).max() < 2e-4 and np.abs(tg - tc).max() < 2e-4, t
     vg, vc = gpu.buffer("volume"), cpu.buffer("volume")
-    fg, wg = _tsdf(vg)
-    fc, wc = _tsdf(vc)
+    fg, wg = gu.tsdf(vg)
+    fc, wc = gu.tsdf(vc)
     tol = 2e-3 if flags else 2e-2      # non-rigid: +-1 LSB bilateral differences move a few removed pixels (whole rays of voxels)
     assert np.mean(wg != wc) < tol
     same = wg == wc
@@ -78,7 +66,7 @@ def test_sequence_matches_oracle(orc, flags):
 def test_first_frame_bit_exact_when_bilateral_is_bypassed(orc):
     """frame 0 only touches dists -> integrate -> extract: those must be bit-identical to the oracle (no expf involved)"""
     from oracle import orc_pipe
-    p = _params(96)
+    p = gu.kinfu_params(96, 0, max_nodes=512, cloud_capacity=400000)
     gpu = kf.KinFu(p)
     cpu = orc_pipe.KinFu(orc_pipe.params_from(p))
     d = synth.umbrella_depth(0)
@@ -92,7 +80,7 @@ def test_first_frame_bit_exact_when_bilateral_is_bypassed(orc):
 
 
 def test_reset_on_tracking_loss_and_recovery():
-    p = _params(32, kf.RIGID_ONLY)
+    p = gu.kinfu_params(32, kf.RIGID_ONLY, max_nodes=512, cloud_capacity=400000)
     k = kf.KinFu(p)
     assert k(synth.sphere_wall_depth(seed=0)) is False
     assert k(synth.sphere_wall_depth(seed=1)) is True
@@ -106,13 +94,13 @@ def test_reset_on_tracking_loss_and_recovery():
 
 
 def test_volume_dims_must_be_multiple_of_32():
-    p = _params(40)
+    p = gu.kinfu_params(40, 0, max_nodes=512, cloud_capacity=400000)
     with pytest.raises(RuntimeError):
         kf.KinFu(p)                                                      # CV_Assert(dims[0] % 32 == 0), kinfu.cpp:97
 
 
 def test_stage_timing_and_launch_count():
-    p = _params(64, kf.STAGE_TIMING)
+    p = gu.kinfu_params(64, kf.STAGE_TIMING, max_nodes=512, cloud_capacity=400000)
     k = kf.KinFu(p)
     for t in range(3):
         k(synth.umbrella_depth(t))
@@ -131,7 +119,7 @@ def test_batch_entry_advances_independent_sequences_concurrently():
     seqs = [[synth.umbrella_depth(t, seed=s) for t in range(frames)] for s in range(n)]
     want, want_nodes = [], []
     for s in range(n):
-        k = kf.KinFu(_params(64))
+        k = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
         for d in seqs[s]:
             k(d)
         want.append(k.state_digest())
@@ -140,7 +128,7 @@ def test_batch_entry_advances_independent_sequences_concurrently():
     ks = []
     for s in range(n):
         torch.cuda.set_device(s % ndev)
-        ks.append(kf.KinFu(_params(64)))
+        ks.append(kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000)))
     torch.cuda.set_device(0)
     lib = ks[0].lib
     handles = (C.c_void_p * n)(*[k.h for k in ks])
@@ -176,7 +164,7 @@ def test_use_depth_loop_tracks_like_the_points_loop():
     frames = [synth.umbrella_depth(t) for t in range(5)]
     runs = {}
     for flags in (0, kf.USE_DEPTH):
-        k = kf.KinFu(_params(64, flags))
+        k = kf.KinFu(gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000))
         vols = []
         for t, d in enumerate(frames):
             assert k(d) == (t > 0)
@@ -199,7 +187,7 @@ def test_f2_solve_in_the_frame_loop():
     checked here only for what must hold: the loop runs, the energy of every frame's solve does not increase, nodes stay finite and the
     rotations move (the translation-only solve leaves them at identity)."""
     import ctypes as C
-    k = kf.KinFu(_params(64, kf.F2_SOLVE))
+    k = kf.KinFu(gu.kinfu_params(64, kf.F2_SOLVE, max_nodes=512, cloud_capacity=400000))
     for t in range(4):
         assert k(synth.umbrella_depth(t)) == (t > 0)
         if t:

@@ -9,22 +9,12 @@ import numpy as np
 ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 
-import mesh_oracle  # noqa: E402
 import raster_oracle  # noqa: E402
-from oracle import orc  # noqa: E402
-from test_mesh import IDENT, sphere_volume  # noqa: E402
-
-# pixel-exact camera: u = fma(32, x / 1, 0) is an integer for x = i / 32 on the plane z = 1
-K_EXACT = (32.0, 32.0, 0.0, 0.0)
-
-
-def _plane_verts(uv):
-    uv = np.asarray(uv, np.float64)
-    return np.stack([uv[:, 0] / 32.0, uv[:, 1] / 32.0, np.ones(len(uv))], 1).astype(np.float32)
+from scenes import IDENT, K_EXACT, SPHERE_COLS, SPHERE_K, SPHERE_ROWS, look_at, plane_verts, sphere_mesh  # noqa: E402
 
 
 def test_quad_sharing_a_diagonal_is_covered_once_with_top_left_edges():
-    verts = _plane_verts([(2, 2), (10, 2), (10, 8), (2, 8)])
+    verts = plane_verts([(2, 2), (10, 2), (10, 8), (2, 8)])
     tris = np.array([[0, 2, 1], [0, 3, 2]], np.int32)            # camera-facing: negative fixed-point area, the diagonal 0-2 in both
     cov = raster_oracle.coverage(verts, tris, IDENT, K_EXACT, 16, 12)
     want = np.zeros((12, 16), np.int32)
@@ -42,7 +32,7 @@ def test_fan_around_a_pixel_centre_covers_it_once():
     c = np.array([20.0, 20.0])
     ring = [c + np.array([5 * np.cos(a), 5 * np.sin(a)]) for a in np.arange(8) * np.pi / 4]
     ring = [np.round(r * 2) / 2 for r in ring]                     # half-pixel positions, exact in 8 sub-pixel bits
-    verts = _plane_verts([c] + ring)
+    verts = plane_verts([c] + ring)
     tris = np.array([[0, 1 + (k + 1) % 8, 1 + k] for k in range(8)], np.int32)
     cov = raster_oracle.coverage(verts, tris, IDENT, K_EXACT, 40, 40)
     assert cov[20, 20] == 1
@@ -51,7 +41,7 @@ def test_fan_around_a_pixel_centre_covers_it_once():
 
 
 def test_reversed_winding_draws_nothing():
-    verts = _plane_verts([(2, 2), (10, 2), (10, 8), (2, 8)])
+    verts = plane_verts([(2, 2), (10, 2), (10, 8), (2, 8)])
     tris = np.array([[0, 1, 2], [0, 2, 3]], np.int32)
     ids, pts, nrm, stats = raster_oracle.raster(verts, tris, IDENT, K_EXACT, 16, 12)
     assert np.all(ids == -1) and np.all(np.isnan(pts)) and np.all(np.isnan(nrm))
@@ -60,7 +50,7 @@ def test_reversed_winding_draws_nothing():
 
 
 def test_skipped_triangles_are_counted():
-    good = _plane_verts([(2, 2), (10, 2), (10, 8)])
+    good = plane_verts([(2, 2), (10, 2), (10, 8)])
     near = good.copy(); near[1, 2] = 0.005                         # c.z < DF_RASTER_NEAR
     guard = good.copy(); guard[1, 0] = 3000.0                      # u = 96000 px: outside the +-2^16 band
     nonfinite = good.copy(); nonfinite[2, 1] = np.inf
@@ -75,7 +65,7 @@ def test_skipped_triangles_are_counted():
 
 
 def test_identical_triangles_the_smaller_index_wins():
-    verts = _plane_verts([(2, 2), (10, 2), (10, 8)])
+    verts = plane_verts([(2, 2), (10, 2), (10, 8)])
     ids, _, _, stats = raster_oracle.raster(verts, [[0, 2, 1]] * 3, IDENT, K_EXACT, 16, 12)
     drawn = ids >= 0
     assert drawn.sum() > 10 and np.all(ids[drawn] == 0)
@@ -88,29 +78,6 @@ def test_identical_triangles_the_smaller_index_wins():
 
 
 # ------------------------------------------------------------------ the analytic sphere ------------------------------------------------------
-SPHERE_K = (150.0, 150.0, 79.5, 59.5)
-SPHERE_COLS, SPHERE_ROWS = 160, 120
-
-
-def sphere_mesh():
-    """the marching-cubes mesh of test_mesh.sphere_volume (float32 [N, 4] cloud, int32 [T, 3]), its centre and radius (m), voxel size"""
-    vol, dims, vsz, trunc, centre, radius = sphere_volume()
-    cloud = orc.extract_cloud(vol, dims, vsz, trunc, 64, IDENT, int(np.prod(dims)) * 3)
-    tris = mesh_oracle.mesh(vol, dims, len(cloud))
-    return np.ascontiguousarray(cloud, np.float32), tris, np.asarray(centre, np.float64), float(radius), float(vsz[0])
-
-
-def look_at(centre, distance, direction=(0.0, 0.0, 1.0)):
-    """world-to-camera (R, t) of a camera `distance` from `centre` looking along `direction` (camera y roughly down the world's y)"""
-    f = np.asarray(direction, np.float64); f /= np.linalg.norm(f)
-    up = np.array([0.0, 1.0, 0.0]) if abs(f[1]) < 0.9 else np.array([1.0, 0.0, 0.0])
-    x = np.cross(up, f); x /= np.linalg.norm(x)
-    y = np.cross(f, x)
-    R = np.stack([x, y, f])                                        # rows: camera axes in world coordinates
-    eye = np.asarray(centre, np.float64) - distance * f
-    return R.astype(np.float32), (-R @ eye).astype(np.float32)
-
-
 def _ray_dirs(K, cols, rows):
     fx, fy, cx, cy = (np.float32(v) for v in K)
     i = np.arange(cols, dtype=np.float32)[None, :]

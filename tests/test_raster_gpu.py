@@ -12,40 +12,16 @@ import pytest
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-from dynamicfusion_b200 import capi, kinfu as kf  # noqa: E402
+from dynamicfusion_b200 import capi, kinfu as kf, synth  # noqa: E402
+import color_oracle as co  # noqa: E402
+import gpu_util as gu  # noqa: E402
 import mesh_oracle  # noqa: E402
 import raster_oracle  # noqa: E402
 from oracle import orc  # noqa: E402
-from test_mesh import IDENT  # noqa: E402
-from test_mesh_gpu import FRAMES, _c1_volume, _params, _run  # noqa: E402
-from test_raster import look_at, sphere_mesh  # noqa: E402
+from scenes import IDENT, K640, look_at, sphere_mesh  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
-K640 = (525.0, 525.0, 319.5, 239.5)
-
-
-def _gpu_raster(verts, tris, w2c, K, cols, rows, with_ids=True):
-    """df_raster_mesh on padded-pitch device maps; returns (tri_ids or None, points, normals, stats) as numpy"""
-    lib = capi.load()
-    s = torch.cuda.current_stream().cuda_stream
-    v = torch.from_numpy(np.ascontiguousarray(verts, np.float32)).cuda()
-    t = torch.from_numpy(np.ascontiguousarray(np.asarray(tris, np.int32).reshape(-1, 3))).cuda()
-    pc = cols + 3                                                        # padded rows: pitches wider than the image
-    pts = torch.full((rows, pc, 4), 7.0, dtype=torch.float32, device="cuda")
-    nrm = torch.full((rows, pc, 4), 7.0, dtype=torch.float32, device="cuda")
-    ids = torch.full((rows, pc), -7, dtype=torch.int32, device="cuda")
-    stats = torch.full((5,), 99, dtype=torch.int64, device="cuda")
-    ws = torch.empty(lib.df_raster_workspace_bytes(len(v), len(t), cols, rows), dtype=torch.uint8, device="cuda")
-    capi.check(lib.df_raster_mesh(v.data_ptr(), len(v), v.shape[1], t.data_ptr() if len(t) else None, len(t), capi.make_aff(*w2c),
-                                  capi.make_intr(*K), cols, rows, ids.data_ptr() if with_ids else None, pc * 4, pts.data_ptr(), pc * 16,
-                                  nrm.data_ptr(), pc * 16, stats.data_ptr(), ws.data_ptr(), s))
-    P, N, I = pts.cpu().numpy(), nrm.cpu().numpy(), ids.cpu().numpy()
-    assert np.all(P[:, cols:] == 7.0) and np.all(N[:, cols:] == 7.0)     # nothing written past the image's columns
-    if with_ids:
-        assert np.all(I[:, cols:] == -7)
-    else:
-        assert np.all(I == -7)
-    return (I[:, :cols] if with_ids else None), P[:, :cols], N[:, :cols], stats.cpu().numpy().view(np.uint64)
+FRAMES = [synth.umbrella_depth(t) for t in range(10)]
 
 
 def _same(got, want):
@@ -61,7 +37,7 @@ def _same(got, want):
 
 def _check(verts, tris, w2c, K, cols, rows):
     want = raster_oracle.raster(verts, tris, w2c, K, cols, rows)
-    _same(_gpu_raster(verts, tris, w2c, K, cols, rows), want)
+    _same(gu.gpu_raster(verts, tris, w2c, K, cols, rows), want)
     return want
 
 
@@ -76,12 +52,12 @@ def test_sphere_from_three_poses_equals_the_oracle():
     # xyz rows (vstride 3) and no index map give the same maps
     w2c = look_at(centre, 0.5, (0.3, -0.2, 1.0))
     want = raster_oracle.raster(cloud, tris, w2c, K640, 640, 480)
-    got = _gpu_raster(np.ascontiguousarray(cloud[:, :3]), tris, w2c, K640, 640, 480, with_ids=False)
+    got = gu.gpu_raster(np.ascontiguousarray(cloud[:, :3]), tris, w2c, K640, 640, 480, with_ids=False)
     _same(got, (None,) + want[1:])
 
 
 def test_canonical_mesh_of_c1_256_equals_the_oracle():
-    vol, dims, vs, trunc = _c1_volume()
+    vol, dims, vs, trunc = gu.c1_volume()
     cloud = orc.extract_cloud(vol, dims, (vs,) * 3, trunc, 64, IDENT, 3 * int(np.prod(dims)))
     tris = mesh_oracle.mesh(vol, dims, len(cloud))
     assert tris is not None and len(tris) > 100000
@@ -93,12 +69,12 @@ def test_canonical_mesh_of_c1_256_equals_the_oracle():
 
 
 def test_live_mesh_after_six_frames_equals_the_oracle():
-    k = _run(FRAMES[:6])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:6])
     assert k.info()["nodes"] >= 8
     v, _, f = k.mesh(live=True)
     R, t = k.getCameraPose()
     k.close()
-    _, _, _, stats = _check(v, f, raster_oracle.aff_inv(R, t), K640, 640, 480)
+    _, _, _, stats = _check(v, f, co.aff_inv((R, t)), K640, 640, 480)
     assert stats[4] > 1000
 
 
@@ -109,9 +85,9 @@ def test_ragged_image_with_off_centre_intrinsics():
 
 def test_empty_mesh_draws_nothing():
     verts = np.zeros((5, 4), np.float32)
-    ids, pts, nrm, stats = _gpu_raster(verts, np.zeros((0, 3), np.int32), IDENT, K640, 64, 48)
+    ids, pts, nrm, stats = gu.gpu_raster(verts, np.zeros((0, 3), np.int32), IDENT, K640, 64, 48)
     assert np.all(ids == -1) and np.all(np.isnan(pts)) and np.all(np.isnan(nrm)) and np.all(stats == 0)
-    ids, pts, nrm, stats = _gpu_raster(np.zeros((0, 4), np.float32), np.zeros((0, 3), np.int32), IDENT, K640, 64, 48)
+    ids, pts, nrm, stats = gu.gpu_raster(np.zeros((0, 4), np.float32), np.zeros((0, 3), np.int32), IDENT, K640, 64, 48)
     assert np.all(ids == -1) and np.all(np.isnan(pts)) and np.all(stats == 0)
 
 
@@ -140,7 +116,7 @@ def _render_dev(k, live):
 
 
 def test_kinfu_render_equals_the_oracle_on_its_mesh():
-    k = _run(FRAMES[:6])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:6])
     p = k.params
     K = (p.intr.fx, p.intr.fy, p.intr.cx, p.intr.cy)
     R, t = k.getCameraPose()
@@ -150,7 +126,7 @@ def test_kinfu_render_equals_the_oracle_on_its_mesh():
         defaults = (None, (np.eye(3, dtype=np.float32), np.zeros(3, np.float32)) if live else (R, t))
         for pose, cam2model in (defaults, (moved, moved)):
             pts, nrm, ids = k.render(pose, live)
-            want = raster_oracle.raster(v, f, raster_oracle.aff_inv(*cam2model), K, p.cols, p.rows)
+            want = raster_oracle.raster(v, f, co.aff_inv(cam2model), K, p.cols, p.rows)
             _same((ids, pts, nrm, None), want)
             assert (ids >= 0).sum() > 1000
     k.close()
@@ -159,7 +135,7 @@ def test_kinfu_render_equals_the_oracle_on_its_mesh():
 @pytest.mark.parametrize("overlap", ["1", "0"])
 def test_rendering_every_frame_changes_nothing(monkeypatch, overlap):
     monkeypatch.setenv("DF_KINFU_OVERLAP_EXTRACT", overlap)
-    a, b = kf.KinFu(_params()), kf.KinFu(_params())
+    a, b = (kf.KinFu(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000)) for _ in range(2))
     for t, d in enumerate(FRAMES[:8]):
         a(d)
         b(d)
@@ -173,14 +149,14 @@ def test_rendering_every_frame_changes_nothing(monkeypatch, overlap):
 
 
 def test_failures_write_nothing():
-    k = _run(FRAMES[:3], flags=kf.RIGID_ONLY)
+    k = gu.run(gu.kinfu_params(128, kf.RIGID_ONLY, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:3])
     assert k.info()["nodes"] < 8
     st, ids, pts, nrm = _render_dev(k, 1)
     assert st != 0 and np.all(ids == -7) and np.all(pts == 7.0) and np.all(nrm == 7.0)
     with pytest.raises(RuntimeError):
         k.render(live=True)
     k.close()
-    k = _run(FRAMES[:4], cloud_capacity=2000)                              # the cloud is cut at 2000 points
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=2000), FRAMES[:4])  # the cloud is cut at 2000 points
     assert k.info()["cloud_points"] == 2000
     before = k.state_digest()
     st, ids, pts, nrm = _render_dev(k, 0)
@@ -189,13 +165,8 @@ def test_failures_write_nothing():
     k.close()
 
 
-def _erode(mask, r=2):
-    from scipy.ndimage import binary_erosion
-    return binary_erosion(mask, structure=np.ones((2 * r + 1, 2 * r + 1), bool), border_value=0)
-
-
 def test_canonical_render_agrees_with_the_loops_raycast():
-    k = _run(FRAMES)
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES)
     p = k.params
     vs = p.volume_size[0] / p.volume_dims[0]
     R, t = k.getCameraPose()
@@ -208,9 +179,9 @@ def test_canonical_render_agrees_with_the_loops_raycast():
     hit_r, hit_m = ~np.isnan(rc[..., 2]), ids >= 0
     # hit masks at least 2 px from either map's silhouette: pixels whose 5 x 5 neighbourhood is all hit or all miss in each map (so a
     # disagreement there is a region, not an edge pixel)
-    uniform = (_erode(hit_r) | _erode(~hit_r)) & (_erode(hit_m) | _erode(~hit_m))
+    uniform = (gu.erode(hit_r) | gu.erode(~hit_r)) & (gu.erode(hit_m) | gu.erode(~hit_m))
     agree = (hit_r == hit_m)[uniform].mean()
-    both = _erode(hit_r) & _erode(hit_m)
+    both = gu.erode(hit_r) & gu.erode(hit_m)
     ray = rc[..., :3] / np.linalg.norm(rc[..., :3], axis=-1, keepdims=True)
     cosine = -np.einsum("ijk,ijk->ij", np.nan_to_num(rn[..., :3]), np.nan_to_num(ray))
     sel = both & (cosine > 0.3)
@@ -224,7 +195,7 @@ def test_canonical_render_agrees_with_the_loops_raycast():
 
 
 def test_render_image_shades_the_render_maps():
-    k = _run(FRAMES[:6])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:6])
     p = k.params
     lib = capi.load()
     s = torch.cuda.current_stream().cuda_stream
@@ -281,7 +252,7 @@ def test_misaligned_pitches_are_refused_without_writing():
         assert st != 0
     torch.cuda.synchronize()
     assert torch.all(buf == 7.0) and torch.all(ids == -7)
-    k = _run(FRAMES[:4])
+    k = gu.run(gu.kinfu_params(128, 0, max_nodes=1024, cloud_capacity=1_000_000), FRAMES[:4])
     p = k.params
     pts = torch.full((p.rows, p.cols + 1, 4), 7.0, dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()

@@ -17,6 +17,7 @@ pytestmark = pytest.mark.gpu
 
 import kfref_cases  # noqa: E402
 from dynamicfusion_b200 import capi, host, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 K = synth.DEFAULT_K
 LIGHT = (0.3, -0.2, -0.5)
@@ -86,17 +87,13 @@ def golden(orc):
     return digests, images
 
 
-def _dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 def test_render_kernels_match_the_reference_code(orc, golden):
     digests, images = golden
     _, pts, nrm, _, _ = scene(orc)
     assert np.count_nonzero(~np.isnan(pts[..., 0])) > 100_000
     light = (C.c_float * 3)(*LIGHT)
     lib = capi.load()
-    p_dev, n_dev = _dev(pts), _dev(nrm)
+    p_dev, n_dev = gu.dev(pts), gu.dev(nrm)
     img = torch.zeros((480, 640, 4), dtype=torch.uint8, device="cuda")
     tan = torch.zeros_like(img)
     capi.check(lib.df_render_image(p_dev.data_ptr(), 640 * 16, n_dev.data_ptr(), 640 * 16, 640, 480, light, img.data_ptr(), 640 * 4, None))
@@ -139,7 +136,7 @@ def test_depth_path_image_ops_match_the_reference_code(orc, golden):
     # cloudToDepth on the oracle's ray-cast points
     _, pts, _, _, _ = scene(orc)
     rc = torch.zeros((480, 640), dtype=torch.int16, device="cuda")
-    p_dev = _dev(pts)
+    p_dev = gu.dev(pts)
     capi.check(lib.df_cloud_to_depth(p_dev.data_ptr(), 640 * 16, 640, 480, rc.data_ptr(), 640 * 2, None))
     assert kfref_cases.digest(host.u16_from_device(rc)) == digests["cloud_to_depth"]
     # ray-cast, depth variant = the points variant of the GPU + cloudToDepth, against the reference's raycast(depth) on the same

@@ -5,29 +5,11 @@ import struct
 from pathlib import Path
 
 import numpy as np
-import pytest
 
 import snapshot_model as sm
+from snapshot_model import lib  # noqa: F401  (a fixture)
 
 ROOT = Path(__file__).resolve().parents[1]
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from dynamicfusion_b200 import build, capi
-    build.build()
-    return capi.load()
-
-
-def _params(capi, lib):
-    p = capi.KinfuParams()
-    lib.df_kinfu_default_params(C.byref(p), 0)
-    p.cols, p.rows = 64, 48
-    for i in range(3):
-        p.volume_dims[i] = (32, 24, 20)[i]
-    p.icp_iter_num[:] = [3, 2, 0, 0]
-    p.cloud_capacity = 1000
-    return p
 
 
 def _snapshot(capi, lib, p, n_poses=2, M=3, cloud=5, payload_words=7):
@@ -45,17 +27,11 @@ def _snapshot(capi, lib, p, n_poses=2, M=3, cloud=5, payload_words=7):
     return sm.header(body) + body
 
 
-def _call(lib, capi, data: bytes):
-    out = capi.KinfuParams()
-    buf = np.frombuffer(data, np.uint8) if data else np.zeros(1, np.uint8)
-    return lib.df_kinfu_snapshot_params(buf.ctypes.data, len(data), C.byref(out)), out
-
-
 def test_valid_snapshot_returns_its_params(lib):
     from dynamicfusion_b200 import capi
-    p = _params(capi, lib)
+    p = sm.small_params(capi, lib, 0)
     snap = _snapshot(capi, lib, p)
-    st, out = _call(lib, capi, snap)
+    st, out = sm.read_params(lib, capi, snap)
     assert st == 0 and bytes(out) == bytes(p)
     from dynamicfusion_b200.kinfu import KinFu
     assert bytes(KinFu.snapshot_params(snap)) == bytes(p)
@@ -63,7 +39,7 @@ def test_valid_snapshot_returns_its_params(lib):
 
 def test_malformed_snapshots_are_rejected(lib):
     from dynamicfusion_b200 import capi
-    p = _params(capi, lib)
+    p = sm.small_params(capi, lib, 0)
     snap = _snapshot(capi, lib, p)
     body = snap[sm.HEADER:]
     bad = {
@@ -85,20 +61,20 @@ def test_malformed_snapshots_are_rejected(lib):
         b2 = body[:off] + sm.COUNTERS.pack(*fields) + body[off + sm.COUNTERS.size:]
         bad[name] = sm.header(b2) + b2
     for name, data in bad.items():
-        st, _ = _call(lib, capi, data)
+        st, _ = sm.read_params(lib, capi, data)
         assert st != 0, name
 
 
 def test_checksum_model_matches_the_library(lib):
     """a snapshot sealed with the numpy checksum is accepted; every single-bit flip of its body is caught"""
     from dynamicfusion_b200 import capi
-    p = _params(capi, lib)
+    p = sm.small_params(capi, lib, 0)
     snap = bytearray(_snapshot(capi, lib, p))
     rng = np.random.default_rng(0)
     for pos in rng.integers(sm.HEADER, len(snap), 16):
         flipped = bytearray(snap)
         flipped[pos] ^= 1 << int(rng.integers(0, 8))
-        assert _call(lib, capi, bytes(flipped))[0] != 0
+        assert sm.read_params(lib, capi, bytes(flipped))[0] != 0
     assert struct.unpack_from("<Q", snap, 24)[0] == sm.checksum(bytes(snap[sm.HEADER:]))
 
 

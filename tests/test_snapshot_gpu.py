@@ -12,18 +12,10 @@ pytestmark = pytest.mark.gpu
 
 import snapshot_model as sm  # noqa: E402
 from dynamicfusion_b200 import capi, kinfu as kf, synth  # noqa: E402
+import gpu_util as gu  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 PARAMS_BYTES = C.sizeof(capi.KinfuParams)
-
-
-def _params(dim, flags=0, max_nodes=512):
-    p = kf.KinFuParams.default_params_dynamicfusion()
-    kf.KinFuParams.set_volume(p, dim, 1.0)
-    p.max_nodes = max_nodes
-    p.cloud_capacity = 400000
-    p.flags = flags
-    return p
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
@@ -69,7 +61,7 @@ def _gpu_unpack(lib, cls, payload, dims, fill):
 
 def _volumes():
     rng = np.random.default_rng(11)
-    k = kf.KinFu(_params(64))
+    k = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for t in range(4):
         k(synth.umbrella_depth(t))
     scene = k.buffer("volume").copy()
@@ -140,7 +132,7 @@ def _same(a, b):
 
 
 def _straight(flags):
-    k = kf.KinFu(_params(64, flags))
+    k = kf.KinFu(gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000))
     states = []
     for d in FRAMES:
         k(d)
@@ -154,7 +146,7 @@ def test_resume_equals_the_uninterrupted_run(flags, tmp_path):
     straight = _straight(flags)
     assert straight[-1]["info"]["resets"] == 0
     for k_stop in (0, 3):
-        a = kf.KinFu(_params(64, flags))
+        a = kf.KinFu(gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000))
         for d in FRAMES[:k_stop + 1]:
             a(d)
         path = tmp_path / f"s{k_stop}.dfsnap"
@@ -175,17 +167,17 @@ def test_resume_equals_the_uninterrupted_run(flags, tmp_path):
 
 def test_f2_solve_restores_exactly_and_keeps_tracking(tmp_path):
     flags = kf.F2_SOLVE
-    a = kf.KinFu(_params(64, flags))
+    a = kf.KinFu(gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000))
     poses = []
     for d in FRAMES:
         a(d)
         poses.append(np.concatenate([x.reshape(-1) for x in a.getCameraPose()]))
     a.close()
-    a = kf.KinFu(_params(64, flags))
+    a = kf.KinFu(gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:4]:
         a(d)
     snap = a.snapshot()
-    b = kf.KinFu(_params(64, flags))
+    b = kf.KinFu(gu.kinfu_params(64, flags, max_nodes=512, cloud_capacity=400000))
     b.restore(snap)
     assert b.snapshot() == snap
     _same(_state(b), _state(a))
@@ -197,13 +189,13 @@ def test_f2_solve_restores_exactly_and_keeps_tracking(tmp_path):
 
 
 def test_snapshot_after_a_tracking_loss_resumes_into_a_first_frame(tmp_path):
-    a = kf.KinFu(_params(64))
+    a = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:3]:
         a(d)
     assert a(np.zeros((480, 640), np.uint16)) is False                 # ICP degenerate -> reset
     assert a.info()["frame_counter"] == 0 and a.info()["resets"] == 1
     snap = a.snapshot()
-    b = kf.KinFu(_params(64))
+    b = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     b.restore(snap)
     assert (a(FRAMES[3]), b(FRAMES[3])) == (False, False)              # both take the first-frame path
     _same(_state(b), _state(a))
@@ -213,14 +205,14 @@ def test_snapshot_after_a_tracking_loss_resumes_into_a_first_frame(tmp_path):
 
 
 def test_loading_over_another_sequence_equals_loading_into_a_fresh_object():
-    a = kf.KinFu(_params(64))
+    a = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:4]:
         a(d)
     snap = a.snapshot()
-    used = kf.KinFu(_params(64))
+    used = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for t in range(5):
         used(synth.umbrella_depth(t, seed=7))
-    fresh = kf.KinFu(_params(64))
+    fresh = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     used.restore(snap)
     fresh.restore(snap)
     assert used.snapshot() == fresh.snapshot() == snap
@@ -233,13 +225,13 @@ def test_snapshot_resumes_on_another_device():
     if torch.cuda.device_count() < 2:
         pytest.skip("one GPU")
     straight = _straight(0)
-    a = kf.KinFu(_params(64))
+    a = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:4]:
         a(d)
     snap = a.snapshot()
     a.close()
     with torch.cuda.device(1):
-        b = kf.KinFu(_params(64))
+        b = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
         b.restore(snap)
         for t in range(4, 8):
             assert b(FRAMES[t])
@@ -248,11 +240,11 @@ def test_snapshot_resumes_on_another_device():
 
 
 def test_rejected_snapshots_leave_the_object_untouched():
-    a = kf.KinFu(_params(64))
+    a = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:3]:
         a(d)
     snap = a.snapshot()
-    target = kf.KinFu(_params(64))
+    target = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:2]:
         target(d)
     before, before_snap = target.state_digest(), target.snapshot()
@@ -261,7 +253,7 @@ def test_rejected_snapshots_leave_the_object_untouched():
     three = bytearray(snap); three[classes_at + 10] = 3
     flipped = bytearray(snap); flipped[-5] ^= 0x10
     bad = {"truncated": snap[:-1], "flipped payload byte": bytes(flipped), "class byte 3": sm.reseal(bytes(three))}
-    other = kf.KinFu(_params(96))
+    other = kf.KinFu(gu.kinfu_params(96, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:2]:
         other(d)
     other_snap = other.snapshot()
@@ -281,7 +273,7 @@ def test_rejected_snapshots_leave_the_object_untouched():
 
 
 def test_two_saves_of_the_same_state_are_identical():
-    a = kf.KinFu(_params(64))
+    a = kf.KinFu(gu.kinfu_params(64, 0, max_nodes=512, cloud_capacity=400000))
     for d in FRAMES[:5]:
         a(d)
     s1 = a.snapshot()

@@ -9,6 +9,7 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import host, synth  # noqa: E402
+from kfref_cases import _tilted_pose  # noqa: E402
 
 K = synth.DEFAULT_K
 
@@ -23,13 +24,6 @@ def _setup(dim, size, depth, pose=None):
     vol.setGradientDeltaFactor(0.5)
     vol.clear()
     return vol
-
-
-def _tilted_pose():
-    a, b = np.deg2rad(7.0), np.deg2rad(-4.0)
-    Rx = np.array([[1, 0, 0], [0, np.cos(a), -np.sin(a)], [0, np.sin(a), np.cos(a)]])
-    Ry = np.array([[np.cos(b), 0, np.sin(b)], [0, 1, 0], [-np.sin(b), 0, np.cos(b)]])
-    return (Rx @ Ry).astype(np.float32), np.array([0.03, -0.02, 0.05], np.float32)
 
 
 @pytest.mark.parametrize("dim,pose_kind", [(64, "identity"), (128, "tilted"), (96, "tilted")])
