@@ -118,6 +118,8 @@ PROTOTYPES = {
     "df_integrate_warped_workspace_bytes": (_sz, [_i, _i, _i]),
     "df_integrate_warped_launch_count": (_i, []),
     "df_integrate_warped": (_i, [Volume, _vp, _sz, _i, _i, Aff3f, Aff3f, Intr, _vp, _i, _vp, _f, _vp, _vp, _vp, _vp]),
+    "df_integrate_warped_color": (_i, [Volume, _vp, _sz, _i, _i, Aff3f, Aff3f, Intr, _vp, _i, _vp, _f, _vp, _vp, _vp, _vp, _vp, _sz,
+                                       C.POINTER(ColorCamera), C.POINTER(Lens), _vp, _sz, _vp]),
     "df_solve_workspace_bytes": (_sz, [_i, _i]),
     "df_solve_knn_buffers": (_i, [_vp, _i, _i, C.POINTER(_vp), C.POINTER(_vp)]),
     "df_solve_normal_system": (_i, [_vp, _i, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp)]),

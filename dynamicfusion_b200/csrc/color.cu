@@ -56,16 +56,6 @@ __device__ __forceinline__ bool color_gate(const ColorParams &p, int x, int y, i
     });
 }
 
-// integer running average of one voxel word (R, G, B, W) with the sample s (B, G, R, x)
-__device__ __forceinline__ uint32_t color_update(uint32_t c, uchar4 s, int wcap)
-{
-    const uint32_t W = c >> 24, n = W + 1, h = n >> 1;
-    const uint32_t r = ((c & 0xffu) * W + s.z + h) / n;
-    const uint32_t g = (((c >> 8) & 0xffu) * W + s.y + h) / n;
-    const uint32_t b = (((c >> 16) & 0xffu) * W + s.x + h) / n;
-    return r | (g << 8) | (b << 16) | (min(n, (uint32_t)wcap) << 24);
-}
-
 // the walk both integrate kernels share: gate(x, y, z, s) gives voxel (x, y, z)'s sample or skips it; one read-modify-write per changed quad
 template <int VX, class Gate> __device__ __forceinline__ void color_walk(const VolumeWalk &w, const ColorParams &p, Gate gate)
 {
@@ -105,31 +95,6 @@ __global__ void __launch_bounds__(WALK_THREADS) integrate_color_kernel(const Vol
 
 // ---- a colour camera with its own calibration (df_color_depth_map, df_integrate_color_camera) -------------------------------------
 
-struct CameraParams {
-    Aff d2c;                         // depth camera frame -> colour camera frame
-    float fx, fy, cx, cy;            // colour intrinsics
-    float fcols, frows;              // colour image size
-    int cell;                        // colour pixels per map cell and axis
-};
-
-// the depth pixel's point in the colour camera and its colour pixel (u, v): false when it does not land in the colour image.  LENS: through
-// the colour camera's lens (lens.cuh); the instances without it ignore `lens` and are the pinhole projection
-template <bool LENS>
-__device__ __forceinline__ bool to_color(const CameraParams &c, const df_lens &lens, const float3 pd, float3 &pc, float &u, float &v)
-{
-    pc = aff_mul(c.d2c, pd);
-    if constexpr (LENS) {
-        float xd, yd;
-        if (!lens_distort(lens, pc.x / pc.z, pc.y / pc.z, xd, yd)) return false;
-        u = __fmaf_rn(c.fx, xd, c.cx);
-        v = __fmaf_rn(c.fy, yd, c.cy);
-    } else {
-        u = __fmaf_rn(c.fx, pc.x / pc.z, c.cx);
-        v = __fmaf_rn(c.fy, pc.y / pc.z, c.cy);
-    }
-    return pc.z > 0 && u >= 0 && v >= 0 && u < c.fcols && v < c.frows;   // a NaN fails every comparison
-}
-
 template <bool LENS>
 __global__ void __launch_bounds__(256) color_depth_map_kernel(const unsigned short *depth, size_t dpitch, int cols, int rows, float finvx, float finvy,
                                                               float dcx, float dcy, const CameraParams c, uint32_t *map, size_t mpitch,
@@ -146,28 +111,6 @@ __global__ void __launch_bounds__(256) color_depth_map_kernel(const unsigned sho
     float u, v;
     if (!to_color<LENS>(c, lens, pd, pc, u, v)) return;
     atomicMin(row_ptr(map, mpitch, (int)v / c.cell) + (int)u / c.cell, __float_as_uint(pc.z));   // positive floats order as their bits
-}
-
-struct OcclusionParams {
-    CameraParams cam;
-    const uint32_t *map; size_t mpitch;
-    float tol;                       // DF_COLOR_OCCLUSION * trunc_dist
-};
-
-// the colour camera's pixel of the depth-frame point vc: its colour projection and the occlusion test, then the pixel of bgra; false where
-// the camera does not see vc (df_integrate_color_camera's voxels, df_frame_intensity's level-0 points)
-template <bool LENS>
-__device__ __forceinline__ bool camera_sample(const OcclusionParams &o, const df_lens &lens, const uchar4 *bgra, size_t cpitch, float3 vc, uchar4 &smp)
-{
-    float3 pc;
-    float u, v;
-    if (!to_color<LENS>(o.cam, lens, vc, pc, u, v)) return false;
-    const int iu = (int)u, iv = (int)v;
-    const uint32_t zmin = __ldg(row_ptr(o.map, o.mpitch, iv / o.cam.cell) + iu / o.cam.cell);
-    if (zmin == 0xffffffffu) return false;                         // no depth pixel lands in this cell
-    if (pc.z > __uint_as_float(zmin) + o.tol) return false;        // the colour camera sees something nearer here
-    smp = __ldg(row_ptr(bgra, cpitch, iv) + iu);
-    return true;
 }
 
 // the colour camera's sample for voxel (x, y, z): the depth-side gate, then the colour projection and the occlusion test
@@ -341,16 +284,6 @@ extern "C" int df_color_map_dims(df_intr intr, df_color_camera cam, int *map_col
     if (map_cols) *map_cols = (cam.cols + c - 1) / c;
     if (map_rows) *map_rows = (cam.rows + c - 1) / c;
     return 0;
-}
-
-static CameraParams camera_params(const df_color_camera &cam, int cell)
-{
-    CameraParams c;
-    c.d2c = make_aff(cam.depth_to_color);
-    c.fx = cam.intr.fx; c.fy = cam.intr.fy; c.cx = cam.intr.cx; c.cy = cam.intr.cy;
-    c.fcols = (float)cam.cols; c.frows = (float)cam.rows;
-    c.cell = cell;
-    return c;
 }
 
 // the lens argument of a _lens entry: `use` is false for NULL and for the zero lens (the pinhole instances); an invalid lens is refused

@@ -26,6 +26,7 @@
 //        voxel, seed the branch-and-bound (knn8_bvh_seeded) so that it prunes with a near-final bound from the first box on and inserts only
 //        the few nodes that actually changed.  Results are ranked by (distance, index) on every path: identical to the exhaustive scan.
 #include "warp_common.cuh"
+#include "color_sample.cuh"
 #include <cmath>
 #include <cstdlib>
 
@@ -64,6 +65,19 @@ struct FusionParams {
     int use_list;                          // candidate lists per warp run (round 2, see integrate_warped_body); 0: branch-and-bound per voxel only
     float half_diag;                       // upper bound on the distance (world space) from a run's centre to any of its voxel centres
     float half_diag_block;                 // the same for the block's 32 x 8 x zchunk region
+};
+
+// The colour side of df_integrate_warped_color: kColor selects what a warped voxel in the band samples (WC_NONE: no colour side at all --
+// df_integrate_warped's instances); kLens (WC_CAMERA only) projects through the colour camera's lens, as color.cu's LENS instances do.
+enum { WC_NONE = 0, WC_REGISTERED = 1, WC_CAMERA = 2 };
+
+struct WarpedColorParams {
+    uint32_t *colors;                      // the colour volume, laid out as the TSDF volume
+    const uchar4 *bgra; size_t cpitch;     // the frame's colour image: registered to the depth (cols x rows) or the colour camera's
+    float band;                            // DF_COLOR_BAND * trunc_dist
+    int wcap;                              // min(max_weight, 255)
+    OcclusionParams o;                     // WC_CAMERA: the colour camera, the frame's df_color_depth_map and DF_COLOR_OCCLUSION * trunc_dist
+    unsigned long long *counter;           // optional (the entry's counters[2]): += voxels that took a colour sample
 };
 
 // metric depth maxima per FUS_TILE x FUS_TILE pixel tile
@@ -264,8 +278,8 @@ __device__ __noinline__ void fusion_tree_search(const void *grid, const float4 *
     for (int k = 0; k < 8; ++k) { bi_out[k] = bi[k]; bd_out[k] = bd[k]; }
 }
 
-template <bool kIdentity>
-__device__ __forceinline__ void integrate_warped_body(const FusionParams &p)
+template <bool kIdentity, int kColor = WC_NONE, bool kLens = false>
+__device__ __forceinline__ void integrate_warped_body(const FusionParams &p, const WarpedColorParams *wc = nullptr, const df_lens *lens = nullptr)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int xw = blockIdx.x * 32 + (warp & 3) * 8, yw = blockIdx.y * 8 + (warp >> 2) * 4;       // the warp's 8 x 4 voxel footprint
@@ -363,7 +377,7 @@ __device__ __forceinline__ void integrate_warped_body(const FusionParams &p)
 
     int prev[8];
     bool have_prev = false;
-    unsigned int n_upd = 0, n_warp = 0;
+    unsigned int n_upd = 0, n_warp = 0, n_col = 0;
     const size_t slice = (size_t)p.Dx * p.Dy;
     for (int za = z0; za < z1; za += FUS_SUB) {
         const int zb = min(z1, za + FUS_SUB);
@@ -512,6 +526,23 @@ __device__ __forceinline__ void integrate_warped_body(const FusionParams &p)
                 if (vox_negative(val)) brick_mark(p.bricks, x, y, z);
             }
             ++n_upd;
+            if constexpr (kColor != WC_NONE) {
+                // df_integrate_warped_color's rule, on the values the TSDF side just formed: the warped point (tx, ty, tz), its depth pixel
+                // ((int)u, (int)v) and rho.  The band |rho| <= DF_COLOR_BAND * trunc lies inside the TSDF gate rho > -trunc, so every voxel
+                // that can take a colour sample has been written above; the culling (runs skipped when rho < -trunc for all of their voxels
+                // whatever the field does) is conservative for the TSDF and therefore for the colour too.
+                if (fabsf(rho) <= wc->band) {
+                    uchar4 smp;
+                    bool ok = true;
+                    if constexpr (kColor == WC_REGISTERED) smp = __ldg(row_ptr(wc->bgra, wc->cpitch, (int)v) + (int)u);
+                    else ok = camera_sample<kLens>(wc->o, *lens, wc->bgra, wc->cpitch, make_float3(tx, ty, tz), smp);
+                    if (ok) {
+                        uint32_t *cptr = wc->colors + (vptr - p.data);
+                        *cptr = color_update(*cptr, smp, wc->wcap);
+                        ++n_col;
+                    }
+                }
+            }
         }
     }
     if (p.counters) {
@@ -520,6 +551,13 @@ __device__ __forceinline__ void integrate_warped_body(const FusionParams &p)
         if (lane == 0) {
             if (n_upd) atomicAdd(p.counters, (unsigned long long)n_upd);
             if (n_warp) atomicAdd(p.counters + 1, (unsigned long long)n_warp);
+        }
+    }
+    if constexpr (kColor != WC_NONE) {
+        if (wc->counter) {
+            __syncwarp();
+            for (int o = 16; o > 0; o >>= 1) n_col += __shfl_xor_sync(0xffffffffu, n_col, o);
+            if (lane == 0 && n_col) atomicAdd(wc->counter, (unsigned long long)n_col);
         }
     }
 }
@@ -534,6 +572,16 @@ __global__ void __launch_bounds__(256, kMinBlocks) integrate_warped_kernel(const
     DF_PDL_ENTRY();
     if ((__ldg(p.ws + 2) != 0.f) != kIdentity) return;
     integrate_warped_body<kIdentity>(p);
+}
+
+// df_integrate_warped_color: the same voxel walk with the colour side compiled in (kColor, kLens), one kernel per mode so that the
+// colourless instances above keep their code.  Launched at kMinBlocks = 4 only: DF_FUSION_MIN_BLOCKS is a tuning knob of those.
+template <bool kIdentity, int kColor, bool kLens>
+__global__ void __launch_bounds__(256, 4) integrate_warped_color_kernel(const FusionParams p, const WarpedColorParams wc, const df_lens lens)
+{
+    DF_PDL_ENTRY();
+    if ((__ldg(p.ws + 2) != 0.f) != kIdentity) return;
+    integrate_warped_body<kIdentity, kColor, kLens>(p, &wc, &lens);
 }
 
 // |R^T R - I|_max: how far a pose's linear part is from a rotation
@@ -564,9 +612,10 @@ extern "C" size_t df_integrate_warped_workspace_bytes(int cols, int rows, int M)
 
 extern "C" int df_integrate_warped_launch_count(void) { return 4; }
 
-extern "C" int df_integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_pitch, int cols, int rows, df_aff3f vol2world,
-                                   df_aff3f world2cam, df_intr intr, const float *nodes, int M, const void *node_grid, float weight_scale,
-                                   unsigned long long *counters, unsigned char *activity, void *workspace, void *stream)
+// both entries: wc == NULL launches df_integrate_warped's kernels, else the colour instances of kColor (lens: WC_CAMERA only, NULL = pinhole)
+static int integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_pitch, int cols, int rows, df_aff3f vol2world, df_aff3f world2cam,
+                            df_intr intr, const float *nodes, int M, const void *node_grid, float weight_scale, unsigned long long *counters,
+                            unsigned char *activity, void *workspace, const WarpedColorParams *wc, int kColor, const df_lens *lens, void *stream)
 {
     if (!node_grid || !nodes || M <= 0 || !vol.data || !depth) return (int)cudaErrorInvalidValue;
     cudaStream_t s = (cudaStream_t)stream;
@@ -642,7 +691,19 @@ extern "C" int df_integrate_warped(df_volume vol, const uint16_t *depth, size_t 
     launch_pdl(fusion_prepare_kernel, dim3(2), dim3(256), 0, s, ws, p.tiles_x, p.tiles_y, p.ctiles_x, p.ctiles_y, nodes, M, rec);
     dim3 grid(div_up(vol.dims[0], 32), div_up(vol.dims[1], 8), div_up(vol.dims[2], p.zchunk));
     static const int min_blocks = [] { const char *e = getenv("DF_FUSION_MIN_BLOCKS"); return (e && atoi(e) == 3) ? 3 : 4; }();
-    if (min_blocks == 4) {
+    if (wc) {
+        const df_lens L = lens ? *lens : df_lens{};
+        if (kColor == WC_REGISTERED) {
+            launch_pdl(integrate_warped_color_kernel<true, WC_REGISTERED, false>, grid, dim3(256), 0, s, p, *wc, L);
+            launch_pdl(integrate_warped_color_kernel<false, WC_REGISTERED, false>, grid, dim3(256), 0, s, p, *wc, L);
+        } else if (!lens) {
+            launch_pdl(integrate_warped_color_kernel<true, WC_CAMERA, false>, grid, dim3(256), 0, s, p, *wc, L);
+            launch_pdl(integrate_warped_color_kernel<false, WC_CAMERA, false>, grid, dim3(256), 0, s, p, *wc, L);
+        } else {
+            launch_pdl(integrate_warped_color_kernel<true, WC_CAMERA, true>, grid, dim3(256), 0, s, p, *wc, L);
+            launch_pdl(integrate_warped_color_kernel<false, WC_CAMERA, true>, grid, dim3(256), 0, s, p, *wc, L);
+        }
+    } else if (min_blocks == 4) {
         launch_pdl(integrate_warped_kernel<true, 4>, grid, dim3(256), 0, s, p);
         launch_pdl(integrate_warped_kernel<false, 4>, grid, dim3(256), 0, s, p);
     } else {
@@ -652,4 +713,43 @@ extern "C" int df_integrate_warped(df_volume vol, const uint16_t *depth, size_t 
     if (own) cudaFreeAsync(ws, s);
     DF_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int df_integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_pitch, int cols, int rows, df_aff3f vol2world,
+                                   df_aff3f world2cam, df_intr intr, const float *nodes, int M, const void *node_grid, float weight_scale,
+                                   unsigned long long *counters, unsigned char *activity, void *workspace, void *stream)
+{
+    return integrate_warped(vol, depth, depth_pitch, cols, rows, vol2world, world2cam, intr, nodes, M, node_grid, weight_scale, counters, activity,
+                            workspace, nullptr, WC_NONE, nullptr, stream);
+}
+
+extern "C" int df_integrate_warped_color(df_volume vol, const uint16_t *depth, size_t depth_pitch, int cols, int rows, df_aff3f vol2world,
+                                         df_aff3f world2cam, df_intr intr, const float *nodes, int M, const void *node_grid, float weight_scale,
+                                         unsigned long long *counters, unsigned char *activity, void *workspace, uint32_t *colors, const void *bgra,
+                                         size_t bgra_pitch, const df_color_camera *cam, const df_lens *lens, const uint32_t *map, size_t map_pitch,
+                                         void *stream)
+{
+    if (!node_grid || !nodes || M <= 0 || !vol.data || !depth || !colors || !bgra || cols <= 0 || rows <= 0 || vol.dims[0] <= 0 || vol.dims[1] <= 0 ||
+        vol.dims[2] <= 0 || depth_pitch < (size_t)cols * 2 || depth_pitch % 2 || bgra_pitch % 4)
+        return (int)cudaErrorInvalidValue;
+    WarpedColorParams wc = {};
+    wc.colors = colors;
+    wc.bgra = (const uchar4 *)bgra; wc.cpitch = bgra_pitch;
+    wc.band = DF_COLOR_BAND * vol.trunc_dist;
+    wc.wcap = vol.max_weight < 255 ? vol.max_weight : 255;
+    wc.counter = counters ? counters + 2 : nullptr;
+    bool use_lens = false;
+    if (cam) {
+        int mcols = 0, mrows = 0, cell = 0;
+        if (df_color_map_dims(intr, *cam, &mcols, &mrows, &cell) || !map || map_pitch < (size_t)mcols * 4 || map_pitch % 4 ||
+            bgra_pitch < (size_t)cam->cols * 4 || (lens && df_lens_check(*lens)))
+            return (int)cudaErrorInvalidValue;
+        use_lens = lens && !lens_is_zero(*lens);
+        wc.o.cam = camera_params(*cam, cell);
+        wc.o.map = map; wc.o.mpitch = map_pitch;
+        wc.o.tol = DF_COLOR_OCCLUSION * vol.trunc_dist;
+    } else if (bgra_pitch < (size_t)cols * 4)
+        return (int)cudaErrorInvalidValue;
+    return integrate_warped(vol, depth, depth_pitch, cols, rows, vol2world, world2cam, intr, nodes, M, node_grid, weight_scale, counters, activity,
+                            workspace, &wc, cam ? WC_CAMERA : WC_REGISTERED, use_lens ? lens : nullptr, stream);
 }

@@ -521,9 +521,21 @@ int dynamicfusion(KinFu &k, const Img &depth, const Img &live_pts, const float *
         // the field solved above and fused against the (bilateral-filtered) frame; no pixel is removed, no rigid integrate.
         mark(k, 7);
         unsigned long long *counter = (p.flags & DF_KINFU_STAGE_TIMING) ? k.n_upd.p : nullptr;
-        if (counter) cudaMemsetAsync(counter, 0, 16, s);
-        CK(df_integrate_warped(vol_of(k), (const uint16_t *)depth.ptr, depth.pitch, p.cols, p.rows, p.volume_pose, to_aff(inv_pose),
-                               p.intr, k.nodes, k.M, k.node_grid, p.fusion_weight_scale, counter, k.activity, k.fusion_ws, s));
+        // write-after-read: the previous frame's extraction (deferred to the auxiliary stream) reads the volume, the activity map and the
+        // colour volume this step writes
+        if (int w = wait_extract_on_main(k)) return w;
+        if ((p.flags & DF_KINFU_WARPED_COLOR) && k.frame_bgra) {
+            // DF_KINFU_WARPED_COLOR: the frame's colours go in during the same voxel walk, each voxel sampled where the field carries it
+            if (counter) cudaMemsetAsync(counter, 0, 24, s);
+            CK(df_integrate_warped_color(vol_of(k), (const uint16_t *)depth.ptr, depth.pitch, p.cols, p.rows, p.volume_pose, to_aff(inv_pose),
+                                         p.intr, k.nodes, k.M, k.node_grid, p.fusion_weight_scale, counter, k.activity, k.fusion_ws, k.color_vol,
+                                         k.frame_bgra, k.frame_bgra_pitch, k.has_cam ? &k.cam : nullptr, color_lens_of(k),
+                                         (const uint32_t *)k.color_map.ptr, k.color_map.pitch, s));
+        } else {
+            if (counter) cudaMemsetAsync(counter, 0, 16, s);
+            CK(df_integrate_warped(vol_of(k), (const uint16_t *)depth.ptr, depth.pitch, p.cols, p.rows, p.volume_pose, to_aff(inv_pose),
+                                   p.intr, k.nodes, k.M, k.node_grid, p.fusion_weight_scale, counter, k.activity, k.fusion_ws, s));
+        }
         k.launches += df_integrate_warped_launch_count();
     } else {
         // surface_fusion (tsdf_volume.cpp:228-255): psdf projects the warped vertices into the (bilateral-filtered) depth,
@@ -686,6 +698,8 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         }
         const char *xr = getenv("DF_EXTEND_RADIUS");
         if (xr) k->p.extend_radius = (float)atof(xr);
+        const char *wc = getenv("DF_KINFU_WARPED_COLOR");                  // for objects with both flags it needs only
+        if (wc && atoi(wc) != 0 && (k->p.flags & DF_KINFU_COLOR) && (k->p.flags & DF_KINFU_WARPED_INTEGRATE)) k->p.flags |= DF_KINFU_WARPED_COLOR;
         const char *ct = getenv("DF_KINFU_COLOR_TRACKING");                // for colour objects only: a colourless one stays as it was
         if (ct && atoi(ct) != 0 && (k->p.flags & DF_KINFU_COLOR)) k->p.flags |= DF_KINFU_COLOR_TRACKING;
         const char *rb = getenv("DF_RAYCAST_BRICKS");
@@ -694,9 +708,16 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         if (w) k->p.fusion_weight_scale = (float)atof(w);
     }
     const df_kinfu_params &p = k->p;
-    if ((p.flags & DF_KINFU_COLOR) && (p.flags & DF_KINFU_WARPED_INTEGRATE)) {
-        fprintf(stderr, "df_kinfu_create: DF_KINFU_COLOR cannot be combined with DF_KINFU_WARPED_INTEGRATE: under per-voxel warped fusion a "
-                        "voxel meets its pixel through the warp field, and colour is not carried through it\n");
+    if ((p.flags & DF_KINFU_WARPED_COLOR) && !((p.flags & DF_KINFU_COLOR) && (p.flags & DF_KINFU_WARPED_INTEGRATE))) {
+        fprintf(stderr, "df_kinfu_create: DF_KINFU_WARPED_COLOR needs %s: it fuses the colour volume during the per-voxel warped fusion\n",
+                !(p.flags & DF_KINFU_COLOR) ? "DF_KINFU_COLOR" : "DF_KINFU_WARPED_INTEGRATE");
+        delete k;
+        return nullptr;
+    }
+    if ((p.flags & DF_KINFU_COLOR) && (p.flags & DF_KINFU_WARPED_INTEGRATE) && !(p.flags & DF_KINFU_WARPED_COLOR)) {
+        fprintf(stderr, "df_kinfu_create: DF_KINFU_COLOR cannot be combined with DF_KINFU_WARPED_INTEGRATE alone: under per-voxel warped fusion a "
+                        "voxel meets its pixel through the warp field, and the rigid colour rule does not follow it; add DF_KINFU_WARPED_COLOR, "
+                        "which carries each voxel's colour sample through the field\n");
         delete k;
         return nullptr;
     }

@@ -260,6 +260,26 @@ class TsdfVolume:
                                               self.activity_.data_ptr() if self.activity_ is not None else None, None, _stream()))
         return world2cam
 
+    def integrate_warped_color(self, depth: torch.Tensor, camera_pose, intr, warp_field, colors: torch.Tensor, bgra: torch.Tensor,
+                               weight_scale: float = 0.0, counters: torch.Tensor | None = None, color_camera=None, lens=None,
+                               color_map: torch.Tensor | None = None):
+        """integrate_warped, and the frame's colours fused into `colors` (int32 [Dx*Dy*Dz], df_integrate_color's words) in the same voxel
+        walk (dfusion.h df_integrate_warped_color).  bgra: uint8 [rows, cols, 4] registered to the depth, or the colour camera's image
+        when color_camera (capi.ColorCamera) is given together with color_map (df_color_depth_map of the same frame) and, optionally, its
+        lens (capi.Lens).  counters (optional, int64 [3]): voxels written, warped, coloured."""
+        world2cam = aff_mul(aff_inv(camera_pose), warp_field.warp_to_live_)
+        rows, cols = depth.shape
+        if warp_field.grid_ is None:
+            raise RuntimeError("integrate_warped_color needs the node grid (WarpField(use_grid=True) + buildKDTree)")
+        capi.check(_lib().df_integrate_warped_color(
+            self._vol(), depth.data_ptr(), cols * 2, cols, rows, capi.make_aff(*self.pose_), capi.make_aff(*world2cam), capi.make_intr(*intr),
+            warp_field.nodes_.data_ptr(), warp_field.nodes_.shape[0], warp_field.grid_.data_ptr(), float(weight_scale),
+            counters.data_ptr() if counters is not None else None, self.activity_.data_ptr() if self.activity_ is not None else None, None,
+            colors.data_ptr(), bgra.data_ptr(), bgra.stride(0) * bgra.element_size(),
+            C.byref(color_camera) if color_camera is not None else None, C.byref(lens) if lens is not None else None,
+            color_map.data_ptr() if color_map is not None else None, color_map.stride(0) * 4 if color_map is not None else 0, _stream()))
+        return world2cam
+
     def raycast(self, camera_pose, intr, cols: int, rows: int, dense: bool = False):
         """dense=True forces the plain march (df_raycast_points) on a tracked volume; by default a tracked volume's march skips the
         bricks without negative voxels (df_raycast_points_tracked) -- same maps bit for bit"""

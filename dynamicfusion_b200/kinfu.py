@@ -25,6 +25,7 @@ WARPED_INTEGRATE = 8      # DF_KINFU_WARPED_INTEGRATE: per-voxel warped fusion (
 COLOR = 256               # DF_KINFU_COLOR: fuse RGB-D frames into a colour volume; coloured cloud, mesh export and mesh render
 LIVE_MODEL = 128          # DF_KINFU_LIVE_MODEL: ICP and the data term's association against the rendered live model, not the canonical ray-casts
 COLOR_TRACKING = 512      # DF_KINFU_COLOR_TRACKING: colour frames are tracked with photometric ICP rows as well (needs COLOR)
+WARPED_COLOR = 1024       # DF_KINFU_WARPED_COLOR: colour fused during per-voxel warped fusion (needs COLOR and WARPED_INTEGRATE)
 
 
 class KinFuParams:

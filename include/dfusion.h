@@ -602,6 +602,31 @@ int df_integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_pitch
                         df_aff3f world2cam, df_intr intr, const float *nodes, int M, const void *node_grid, float weight_scale,
                         unsigned long long *counters, unsigned char *activity, void *workspace, void *stream);
 
+/* df_integrate_warped_color: df_integrate_warped, and in the same voxel walk the frame's colour image fused into the colour volume `colors`
+ * (laid out as vol.data, df_integrate_color's words).  The TSDF volume, the activity map and counters[0..1] are df_integrate_warped's on the
+ * same inputs, bit for bit, with the same launches (df_integrate_warped_launch_count).
+ *   Rule (tests/warped_color_oracle.c, over the per-voxel records of oracle/orc_fusion.c's warped fusion; IEEE round-to-nearest, fma only
+ *                 where written): for every voxel that df_integrate_warped's rule writes, with the values that rule formed -- the warped
+ *                 camera-frame point x_t = (tx, ty, tz), its depth pixel ((int)u, (int)v) and rho = depth_mm * 0.001f - tz -- and after its
+ *                 TSDF update:
+ *   Band          skipped unless |rho| <= DF_COLOR_BAND * trunc_dist (the product is one float).  The band is on warped fusion's z-difference
+ *                 rho, not on the ray length from dists that df_integrate_color's band uses: the voxel reaches its pixel through the field,
+ *                 and rho is what its TSDF sample is made of.  It lies inside the TSDF gate rho > -trunc_dist.
+ *   Sample        cam == NULL: bgra pixel ((int)u, (int)v) of an image registered to the depth (cols x rows).  cam != NULL: x_t through
+ *                 the colour camera as df_integrate_color_camera_lens takes vc: pc = depth_to_color * x_t (its fma chain), the colour pixel
+ *                 (through `lens` when it is neither NULL nor the zero lens), the image bounds, the occlusion test against `map`
+ *                 (df_color_depth_map of the same frame) with DF_COLOR_OCCLUSION * trunc_dist, then the pixel of bgra; a voxel the colour
+ *                 camera does not see is skipped.
+ *   Update        df_integrate_color's integer running average, W' = min(W + 1, min(max_weight, 255)).
+ * counters (optional, device, 3 x u64): [0], [1] as df_integrate_warped's, [2] += voxels that took a colour sample.  bgra: device, pitch a
+ * multiple of 4 and at least its width * 4 (cols, or cam->cols); depth_pitch at least cols * 2, even; map as df_color_depth_map writes it.
+ * A NULL pointer, a bad pitch, an invalid camera (df_color_map_dims) or lens (df_lens_check): cudaErrorInvalidValue, nothing written. */
+int df_integrate_warped_color(df_volume vol, const uint16_t *depth, size_t depth_pitch, int cols, int rows, df_aff3f vol2world,
+                              df_aff3f world2cam, df_intr intr, const float *nodes, int M, const void *node_grid, float weight_scale,
+                              unsigned long long *counters, unsigned char *activity, void *workspace, uint32_t *colors, const void *bgra,
+                              size_t bgra_pitch, const df_color_camera *cam, const df_lens *lens, const uint32_t *map, size_t map_pitch,
+                              void *stream);
+
 /* WarpFieldOptimiser::optimiseWarpData (warp_field_optimiser.hpp:14-17) -> CombinedSolver (CombinedSolver.h:25-110)
  * -> Opt LM/PCG on kfusion/solvers/dynamicfusion.t: translation-only data term solved on the device; node
  * translations are updated in place (encodeTranslation, CombinedSolver.h:189-197).
@@ -718,7 +743,8 @@ typedef struct df_kinfu_params {
                                       bit; a colour frame launches two kernels more (three with a colour camera, df_kinfu_set_color_camera), a
                                       depth-only frame on a colour object one (the cloud's colours).
                                       Without the flag nothing is allocated or launched.  Refused at create (reason on stderr) together with
-                                      DF_KINFU_WARPED_INTEGRATE, where a voxel meets its pixel through the warp field; every other flag combines with it.
+                                      DF_KINFU_WARPED_INTEGRATE unless DF_KINFU_WARPED_COLOR is set too: there a voxel meets its pixel through the warp
+                                      field, which the rigid colour rule does not follow; every other flag combines with it.
                                       Environment: DF_KINFU_COLOR=1. */
 #define DF_KINFU_COLOR_TRACKING 512 /* track colour frames with colour as well as geometry: a frame that carries a colour image builds its intensity pyramid
                                       at the end of pre-processing (df_frame_intensity: `levels` launches, through the colour camera when one is set), and
@@ -731,6 +757,17 @@ typedef struct df_kinfu_params {
                                       DF_KINFU_LIVE_MODEL (their previous maps are not the ray-cast's vertex maps of the canonical volume).  Without the
                                       flag nothing is computed, allocated or launched.  Environment: DF_KINFU_COLOR_TRACKING=1 switches it on for every colour object
                                       (DF_KINFU_COLOR by flag or by its variable); colourless objects are left as they are. */
+#define DF_KINFU_WARPED_COLOR 1024  /* colour under per-voxel warped fusion: with DF_KINFU_COLOR and DF_KINFU_WARPED_INTEGRATE (refused at create without
+                                      either, reason on stderr), a colour frame fused through a warp field calls df_integrate_warped_color instead of
+                                      df_integrate_warped -- the frame's colour image (through the colour camera, its lens and the frame's occlusion
+                                      map when one is set) goes into the colour volume in the same voxel walk, each voxel sampled where the field
+                                      carries it, so surface that moves keeps taking the colour it shows now.  The launches are df_integrate_warped's.
+                                      Rigid frames (the first one, fewer than 8 nodes) keep the rigid colour rule of DF_KINFU_COLOR; depth-only frames
+                                      call df_integrate_warped and leave the colour volume as it was.  Colour never feeds back unless
+                                      DF_KINFU_COLOR_TRACKING is set (which combines with it): poses, volume, nodes and cloud equal those of the same
+                                      run with DF_KINFU_WARPED_INTEGRATE alone, bit for bit.  Snapshots carry the flag in their parameters.
+                                      Environment: DF_KINFU_WARPED_COLOR=1 adds it to every object that has both other flags; others are left as they
+                                      are. */
 
 /* which = 0: KinFuParams::default_params_dynamicfusion (kinfu.cpp:14-49); 1: default_params (kinfu.cpp:55-89) */
 void df_kinfu_default_params(df_kinfu_params *p, int which);
@@ -790,7 +827,9 @@ int df_kinfu_join(void *kinfu);
 int df_kinfu_get_pose(void *kinfu, int time, float *pose12_host);
 /* info[0] frame counter, [1] warp nodes M, [2] extracted cloud points, [3] poses stored, [4] last ICP ok,
  * [5] kernels launched in the last frame (memsets are not counted; DF_KINFU_COLOR adds df_integrate_color, or df_color_depth_map and
- * df_integrate_color_camera with a colour camera, on a colour frame, and df_sample_colors after every extraction; DF_KINFU_COLOR_TRACKING adds
+ * df_integrate_color_camera with a colour camera, on a colour frame, and df_sample_colors after every extraction; with DF_KINFU_WARPED_COLOR a
+ * colour frame fused through the warp field adds only df_color_depth_map with a colour camera (df_integrate_warped_color launches what
+ * df_integrate_warped would); DF_KINFU_COLOR_TRACKING adds
  * df_frame_intensity's launches (one per ICP level) on a colour frame and df_model_intensity on a tracked one; a depth lens adds df_undistort
  * on every frame), [6] resets so far, [7] solver LM iterations (last frame),
  * [8] voxels written by the last integrate (DF_KINFU_STAGE_TIMING only), [9] solver PCG iterations (last frame),

@@ -42,6 +42,7 @@ namespace kfusion
         // not in the reference: opt-in extensions of the fusion step (SURVEY 8f), forwarded to df_kinfu_params; the defaults keep the
         // reference's behaviour.  (The same switches exist as environment variables for an unchanged apps/demo.cpp, dfusion.h.)
         int dfusion_flags = 0;             // DF_KINFU_WARPED_INTEGRATE (8) | DF_KINFU_EXTEND_FIELD (16) | DF_KINFU_COLOR (256) | DF_KINFU_COLOR_TRACKING (512)
+                                           // | DF_KINFU_WARPED_COLOR (1024: with COLOR and WARPED_INTEGRATE, colour fused through the warp field)
         float fusion_weight_scale = 0.f;   // df_integrate_warped's weight quantisation (0: every sample weighs 1)
         float extend_radius = 0.f;         // df_extend_field's support radius in metres (0: 0.03)
     };
