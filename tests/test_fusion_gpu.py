@@ -13,53 +13,7 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from dynamicfusion_b200 import host, synth  # noqa: E402
-
-K = synth.DEFAULT_K
-TRUNC, MAXW = 0.04, 64
-
-
-def _volume(dim, size):
-    vol = host.TsdfVolume((dim, dim, dim), track_activity=True)
-    vol.setTruncDist(TRUNC)
-    vol.setMaxWeight(MAXW)
-    vol.setSize((size, size, size))
-    vol.setPose(synth.volume_pose(size))
-    vol.clear()
-    return vol
-
-
-def _surface_nodes(orc, M, seed, t_scale=0.0, rotate=False, weight=3.0):
-    """nodes scattered on the sphere-and-wall scene, with random translations (and optionally rotations) encoded as the reference's
-    DualQuaternion(translation, rotation) does"""
-    rng = np.random.default_rng(seed)
-    d = rng.normal(size=(M, 3))
-    d /= np.linalg.norm(d, axis=1, keepdims=True)
-    v = (np.array([0.0, 0.0, 1.0]) + 0.25 * d).astype(np.float32)
-    v[::3, 2] = 1.38                                         # a third of them on the wall
-    v[::3, :2] = rng.uniform(-0.45, 0.45, size=(len(v[::3]), 2))
-    nodes = orc.make_nodes(v, weight)
-    lib = orc.load()
-    for i in range(M):
-        if rotate:
-            ang = rng.uniform(-0.05, 0.05, 3).astype(np.float32)
-            t = (rng.uniform(-1, 1, 3) * t_scale).astype(np.float32)
-            rot = np.zeros(4, np.float32)
-            dual = np.zeros(4, np.float32)
-            lib.orc_dq_from_euler(C.c_float(float(t[0])), C.c_float(float(t[1])), C.c_float(float(t[2])), C.c_float(float(ang[0])),
-                                  C.c_float(float(ang[1])), C.c_float(float(ang[2])), C.c_void_p(rot.ctypes.data), C.c_void_p(dual.ctypes.data))
-            nodes[i, 3:7] = rot
-            nodes[i, 7:11] = dual
-        elif t_scale > 0:
-            t = (rng.uniform(-1, 1, 3) * t_scale).astype(np.float32)
-            lib.orc_node_encode_translation(C.c_void_p(nodes[i].ctypes.data), C.c_float(float(t[0])), C.c_float(float(t[1])), C.c_float(float(t[2])))
-    return nodes
-
-
-def _tilted_pose():
-    a, b = np.deg2rad(5.0), np.deg2rad(-3.0)
-    Rx = np.array([[1, 0, 0], [0, np.cos(a), -np.sin(a)], [0, np.sin(a), np.cos(a)]])
-    Ry = np.array([[np.cos(b), 0, np.sin(b)], [0, 1, 0], [-np.sin(b), 0, np.cos(b)]])
-    return (Rx @ Ry).astype(np.float32), np.array([0.02, -0.015, 0.03], np.float32)
+from warp_cases import K, MAXW, _surface_nodes, _tilted_pose, _volume  # noqa: E402
 
 
 def _run_both(orc, dim, size, nodes, depth, cam_pose, weight_scale, passes=2):

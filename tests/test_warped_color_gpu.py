@@ -22,7 +22,7 @@ import lens_oracle as lo  # noqa: E402
 import warped_color_oracle as wco  # noqa: E402
 from dynamicfusion_b200 import build, capi, host, synth  # noqa: E402
 from dynamicfusion_b200 import kinfu as kf  # noqa: E402
-from test_fusion_gpu import K, MAXW, _surface_nodes, _tilted_pose, _volume  # noqa: E402
+from warp_cases import K, MAXW, _surface_nodes, _tilted_pose, _volume  # noqa: E402
 
 ROOT = Path(__file__).resolve().parents[1]
 MODES = ["registered", "camera", "camera_lens"]
