@@ -98,7 +98,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 int pdl_enabled();          // DF_PDL (default 1), read once (df_common.cu)
-int knn_warp_list_enabled();   // DF_KNN_WARP_LIST (default 0, A/B): warp-cooperative candidate lists for the 8-NN searches (warp.cu)
 
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args)

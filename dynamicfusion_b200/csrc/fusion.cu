@@ -564,10 +564,10 @@ __device__ __forceinline__ void integrate_warped_body(const FusionParams &p, con
 
 // Two instantiations are launched back to back and the one whose kIdentity does not match the node table returns at once (the flag is a
 // device-side result of fusion_prepare_kernel; reading it on the host would stall the frame loop): each path keeps its own register
-// allocation.  kMinBlocks = 4 (default: 64 registers, a few dozen bytes of spills) or 3 (faster at 512^3 in development); 5 blocks (48 registers,
-// 600 bytes of spills) was much slower.  DF_FUSION_MIN_BLOCKS selects 3.
-template <bool kIdentity, int kMinBlocks>
-__global__ void __launch_bounds__(256, kMinBlocks) integrate_warped_kernel(const FusionParams p)
+// allocation.  4 blocks per SM: 64 registers, a few dozen bytes of spills; 3 blocks (80 registers) was slower at 512^3
+// (integrate stage 12.55 vs 12.48 ms per frame, H100 80GB HBM3 at 700 W), 5 blocks (48 registers, 600 bytes of spills) much slower.
+template <bool kIdentity>
+__global__ void __launch_bounds__(256, 4) integrate_warped_kernel(const FusionParams p)
 {
     DF_PDL_ENTRY();
     if ((__ldg(p.ws + 2) != 0.f) != kIdentity) return;
@@ -575,7 +575,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) integrate_warped_kernel(const
 }
 
 // df_integrate_warped_color: the same voxel walk with the colour side compiled in (kColor, kLens), one kernel per mode so that the
-// colourless instances above keep their code.  Launched at kMinBlocks = 4 only: DF_FUSION_MIN_BLOCKS is a tuning knob of those.
+// colourless instances above keep their code.
 template <bool kIdentity, int kColor, bool kLens>
 __global__ void __launch_bounds__(256, 4) integrate_warped_color_kernel(const FusionParams p, const WarpedColorParams wc, const df_lens lens)
 {
@@ -690,7 +690,6 @@ static int integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_p
     launch_pdl(depth_tile_max_kernel, dim3(p.tiles_x, p.tiles_y), dim3(256), 0, s, depth, depth_pitch, cols, rows, ws + 16, p.tiles_x);
     launch_pdl(fusion_prepare_kernel, dim3(2), dim3(256), 0, s, ws, p.tiles_x, p.tiles_y, p.ctiles_x, p.ctiles_y, nodes, M, rec);
     dim3 grid(div_up(vol.dims[0], 32), div_up(vol.dims[1], 8), div_up(vol.dims[2], p.zchunk));
-    static const int min_blocks = [] { const char *e = getenv("DF_FUSION_MIN_BLOCKS"); return (e && atoi(e) == 3) ? 3 : 4; }();
     if (wc) {
         const df_lens L = lens ? *lens : df_lens{};
         if (kColor == WC_REGISTERED) {
@@ -703,12 +702,9 @@ static int integrate_warped(df_volume vol, const uint16_t *depth, size_t depth_p
             launch_pdl(integrate_warped_color_kernel<true, WC_CAMERA, true>, grid, dim3(256), 0, s, p, *wc, L);
             launch_pdl(integrate_warped_color_kernel<false, WC_CAMERA, true>, grid, dim3(256), 0, s, p, *wc, L);
         }
-    } else if (min_blocks == 4) {
-        launch_pdl(integrate_warped_kernel<true, 4>, grid, dim3(256), 0, s, p);
-        launch_pdl(integrate_warped_kernel<false, 4>, grid, dim3(256), 0, s, p);
     } else {
-        launch_pdl(integrate_warped_kernel<true, 3>, grid, dim3(256), 0, s, p);
-        launch_pdl(integrate_warped_kernel<false, 3>, grid, dim3(256), 0, s, p);
+        launch_pdl(integrate_warped_kernel<true>, grid, dim3(256), 0, s, p);
+        launch_pdl(integrate_warped_kernel<false>, grid, dim3(256), 0, s, p);
     }
     if (own) cudaFreeAsync(ws, s);
     DF_LAUNCH_CHECK();

@@ -102,7 +102,6 @@ struct KinFu {
     float ov_pose[12]; bool has_ov_pose = false;                     // absolute camera pose of the frame
     std::vector<float> ov_nodes; bool has_ov_nodes = false;          // node table after the solve
     df_f2_params f2; DevMem<void> f2_ws;  // DF_KINFU_F2_SOLVE (SURVEY 8f(2))
-    bool raycast_bricks = true;          // DF_RAYCAST_BRICKS=0: dense march (A/B)
     long long solve_overflows = 0;       // frames whose solve was skipped because a normal-matrix row overflowed (solve.cu ROWCAP); info[11]
     long long last_cloud = -1;
     double host_us[4] = {0, 0, 0, 0}; long long host_frames = 0;   // DF_KINFU_HOSTPROF: launch A, ICP wait, launch B, total

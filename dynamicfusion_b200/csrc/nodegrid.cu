@@ -3,14 +3,13 @@
 // set (node vertices are immutable after WarpField::init); one 1024-thread block, deterministic output: nodes are stored
 // cell by cell and, inside a cell, in ascending node index.
 #include "warp_common.cuh"
-#include <cstdlib>
 
 using namespace dfb;
 
 namespace {
 
 __global__ void __launch_bounds__(1024) build_node_grid_kernel(const float *__restrict__ nodes, int M, void *grid, int *cid_tmp, int *order, int *slot,
-                                                               float4 *bvh_box, float4 *bvh_leaf, int L, float spacings_per_cell, int kd_leaves)
+                                                               float4 *bvh_box, float4 *bvh_leaf, int L)
 {
     __shared__ float smin[3][32], smax[3][32];
     __shared__ NodeGridHeader h;
@@ -35,7 +34,7 @@ __global__ void __launch_bounds__(1024) build_node_grid_kernel(const float *__re
         const float ext = fmaxf(fmaxf(hi[0] - lo[0], hi[1] - lo[1]), hi[2] - lo[2]);
         // nodes sample a surface: ~sqrt(M) nodes along the longest extent; ~3 node spacings per cell, so that the 8th
         // neighbour (about 1.7 spacings away) is usually confirmed after the first shell (27 cells)
-        int res = (int)ceilf(sqrtf((float)M) / spacings_per_cell);
+        int res = (int)ceilf(sqrtf((float)M) / 3.0f);
         res = max(1, min(res, NODEGRID_MAX_RES));
         const float cell = ext > 0.f ? ext / (float)res * 1.0001f : 1.f;
         h.ox = lo[0]; h.oy = lo[1]; h.oz = lo[2]; h.cell = cell; h.inv_cell = 1.f / cell;
@@ -120,8 +119,8 @@ __global__ void __launch_bounds__(1024) build_node_grid_kernel(const float *__re
         //    knn8_bvh / knn8_bvh_seeded): leaves = NODEGRID_BVH_LEAF nodes, implicit complete binary tree of L leaves, boxes bottom-up.
         //    Leaf membership = a k-d median split: the entries of every segment (the whole array, then halves, quarters, ... down to 16)
         //    are sorted along the segment's widest axis and the segment is cut in the middle, so a leaf is a compact patch of eight nodes.
-        //    (The first version cut the Morton order into runs of eight: a profile of the fusion kernel showed ~10 leaves entered per query,
-        //    most of its instructions in leaf-entry and box tests -- Z-curve jumps make long, overlapping leaf boxes.)  Segments are aligned
+        //    (Runs of eight in Morton order made long, overlapping leaf boxes at Z-curve jumps: ~10 leaves entered per query of the fusion
+        //    kernel, most of its instructions in leaf-entry and box tests.)  Segments are aligned
         //    power-of-two blocks, so one bitonic network run up to block size S sorts all of them at once; ties break on the node index.
         //    The search result never depends on this order (boxes are built from whatever the leaves hold; ranking is by (distance, index)).
         if (bvh_box) {
@@ -130,10 +129,10 @@ __global__ void __launch_bounds__(1024) build_node_grid_kernel(const float *__re
             const int Mpad = L * NODEGRID_BVH_LEAF;
             for (int sidx = t; sidx < Mpad; sidx += 1024) {
                 float4 e = make_float4(inf, inf, inf, __int_as_float(0x7fffffff));
-                if (sidx < M) { const int i = kd_leaves ? sidx : order[sidx]; const float *v = nodes + (size_t)i * DF_NODE_STRIDE; e = make_float4(v[0], v[1], v[2], __int_as_float(i)); }
+                if (sidx < M) { const float *v = nodes + (size_t)sidx * DF_NODE_STRIDE; e = make_float4(v[0], v[1], v[2], __int_as_float(sidx)); }
                 bvh_leaf[sidx] = e;
             }
-            for (int S = kd_leaves ? Mpad : 0; S >= 2 * NODEGRID_BVH_LEAF; S >>= 1) {       // kd_leaves == 0: runs of the Morton order (first version)
+            for (int S = Mpad; S >= 2 * NODEGRID_BVH_LEAF; S >>= 1) {
                 __syncthreads();
                 // widest axis of every segment (one warp per segment; padding entries are skipped); partial[] holds the axes
                 const int nseg = Mpad / S;
@@ -217,7 +216,7 @@ extern "C" size_t df_node_grid_bytes(int M)
 {
     const size_t ncell = (size_t)NODEGRID_MAX_RES * NODEGRID_MAX_RES * NODEGRID_MAX_RES;
     const size_t m = (size_t)(M > 0 ? M : 1);
-    // header, cell starts, cell-sorted nodes, [BVH boxes + Morton-sorted leaves], cell ids / order / slot
+    // header, cell starts, cell-sorted nodes, [BVH boxes + leaves], cell ids / order / slot
     return 64 + (((ncell + 1) * 4 + 15) & ~(size_t)15) + m * 16 + bvh_bytes((int)m) + 3 * ((m * 4 + 15) & ~(size_t)15) + 256;
 }
 
@@ -234,11 +233,7 @@ extern "C" int df_build_node_grid(const float *nodes, int M, void *grid, void *s
     const int L = bvh_leaves(M);
     float4 *bvh_box = want_order ? reinterpret_cast<float4 *>(tail - bvh_bytes(M)) : nullptr;      // 16-byte aligned: every block above is
     float4 *bvh_leaf = want_order ? bvh_box + 4 * (size_t)L : nullptr;
-    // node spacings per cell (default 3, see the kernel); DF_NODEGRID_SPACINGS overrides
-    static const float spacings = [] { const char *e = getenv("DF_NODEGRID_SPACINGS"); const float v = e ? (float)atof(e) : 3.0f; return v >= 0.5f ? v : 3.0f; }();
-    // BVH leaf membership: 1 = k-d median split (default), 0 = runs of the Morton order (first version); DF_BVH_KD
-    static const int kd_leaves = [] { const char *e = getenv("DF_BVH_KD"); return e ? (int)(atoi(e) != 0) : 1; }();
-    build_node_grid_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(nodes, M, grid, cid_tmp, order, slot, bvh_box, bvh_leaf, L, spacings, kd_leaves);
+    build_node_grid_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(nodes, M, grid, cid_tmp, order, slot, bvh_box, bvh_leaf, L);
     DF_LAUNCH_CHECK();
     return 0;
 }

@@ -176,7 +176,7 @@ int raycast_model(KinFu &k, const float *cam_pose, Img &pts, Img &nrm)
     ++k.launches;
     // the loop's own volume is only ever integrated through the activity map, so the march may skip the bricks without negative voxels
     return df_raycast_points_tracked(vol_of(k), to_aff(cam2vol), Rinv, p.intr, p.cols, p.rows, p.raycast_step_factor, p.gradient_delta_factor,
-                                     (float *)pts.ptr, pts.pitch, (float *)nrm.ptr, nrm.pitch, k.raycast_bricks ? k.activity.p : nullptr, k.stream);
+                                     (float *)pts.ptr, pts.pitch, (float *)nrm.ptr, nrm.pitch, k.activity.p, k.stream);
 }
 
 // compute_points + compute_normals, tsdf_volume.cpp:313-325.  needed_now: the caller reads the cloud right after (first frame: node
@@ -702,8 +702,6 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         if (wc && atoi(wc) != 0 && (k->p.flags & DF_KINFU_COLOR) && (k->p.flags & DF_KINFU_WARPED_INTEGRATE)) k->p.flags |= DF_KINFU_WARPED_COLOR;
         const char *ct = getenv("DF_KINFU_COLOR_TRACKING");                // for colour objects only: a colourless one stays as it was
         if (ct && atoi(ct) != 0 && (k->p.flags & DF_KINFU_COLOR)) k->p.flags |= DF_KINFU_COLOR_TRACKING;
-        const char *rb = getenv("DF_RAYCAST_BRICKS");
-        if (rb && atoi(rb) == 0) k->raycast_bricks = false;
         const char *w = getenv("DF_FUSION_WEIGHT_SCALE");
         if (w) k->p.fusion_weight_scale = (float)atof(w);
     }

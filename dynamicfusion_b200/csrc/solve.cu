@@ -94,11 +94,10 @@ constexpr int PREPARE_THREADS = 256;
 
 __global__ void __launch_bounds__(PREPARE_THREADS, 4) solve_prepare_kernel(const float *__restrict__ nodes, int M, const void *__restrict__ grid,
                                                             const float *__restrict__ canon, const float *__restrict__ live, int N, int stride,
-                                                            SolveWs ws, int cols, int warp_list)
+                                                            SolveWs ws, int cols)
 {
     DF_PDL_ENTRY();
     __shared__ KnnSmem sm;
-    __shared__ float4 knn_wl[PREPARE_THREADS / 32][KNN_WL_CAP];
     const int v = patch_vertex(blockIdx.x, threadIdx.x, cols);      // cols > 0: 8 x 4 pixel patches per warp (solve_fill maps the same way)
     float3 c = make_float3(0.f, 0.f, 0.f), l = c;
     bool valid = false, valid_c = false;       // valid_c: the vertex can be queried; valid: the row enters the solve
@@ -109,8 +108,7 @@ __global__ void __launch_bounds__(PREPARE_THREADS, 4) solve_prepare_kernel(const
         valid = valid_c && !(isnan(l.x) || isnan(l.y) || isnan(l.z));
     }
     int bi[8]; float bd[8];
-    if (grid && warp_list) knn8_grid_warp(grid, valid_c, c.x, c.y, c.z, knn_wl[threadIdx.x >> 5], bi, bd);
-    else if (grid) knn8_grid(grid, valid_c, c.x, c.y, c.z, bi, bd);
+    if (grid) knn8_grid(grid, valid_c, c.x, c.y, c.z, bi, bd);
     else knn8_scan(nodes, M, valid_c, c.x, c.y, c.z, sm, bi, bd);
     double half_b2 = 0.0;
     if (v < N) {
@@ -285,7 +283,7 @@ __device__ __forceinline__ int rows_find_slot(const int *keys, int j)
     return 0;
 }
 
-__global__ void __launch_bounds__(ROWS_THREADS) solve_rows_kernel(SolveWs ws, int M, int N, int quirk, int lpt, int only_if_flag)
+__global__ void __launch_bounds__(ROWS_THREADS) solve_rows_kernel(SolveWs ws, int M, int N, int quirk, int only_if_flag)
 {
     DF_PDL_ENTRY();
     if (only_if_flag && ws.flags[2] == 0) return;
@@ -296,7 +294,7 @@ __global__ void __launch_bounds__(ROWS_THREADS) solve_rows_kernel(SolveWs ws, in
     __shared__ double priv[ROWS_WARPS][ROWS_PRIV];
     __shared__ int nlist;
     __shared__ double red[3][ROWS_WARPS];
-    const int i = lpt ? ws.row_order[blockIdx.x] : (int)blockIdx.x;
+    const int i = ws.row_order[blockIdx.x];
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
     for (int s = tid; s < HCAP; s += ROWS_THREADS) { keys[s] = -1; vals[s] = 0.0; }
@@ -605,7 +603,7 @@ constexpr int RT_WARPS = RT_THREADS / 32;
 constexpr int RT_HCAP = 256;                 // hash slots per row; rows with more than 3/4 of them in use go to the per-entry kernels
 constexpr int RT_LIST = 4096;                // tiles per node kept in shared memory; longer lists are re-read from the byte map
 
-__global__ void __launch_bounds__(RT_THREADS) solve_rows_tiles_kernel(SolveWs ws, int M, int N, int quirk, int lpt)
+__global__ void __launch_bounds__(RT_THREADS) solve_rows_tiles_kernel(SolveWs ws, int M, int N, int quirk)
 {
     DF_PDL_ENTRY();
     __shared__ int keys[RT_HCAP];
@@ -620,7 +618,7 @@ __global__ void __launch_bounds__(RT_THREADS) solve_rows_tiles_kernel(SolveWs ws
     if (tid == 0) skip = ws.flags[2];                    // a tile (or an earlier row) overflowed: fill + rows behind this kernel take the frame
     __syncthreads();                                     // (one reader: other blocks may raise the flag while this one starts)
     if (skip) return;
-    const int i = lpt ? ws.row_order[blockIdx.x] : (int)blockIdx.x;
+    const int i = ws.row_order[blockIdx.x];
     const int NT = ws.ntiles;
     for (int s = tid; s < RT_HCAP; s += RT_THREADS) keys[s] = -1;
     for (int s = tid; s < RT_WARPS * RT_HCAP; s += RT_THREADS) (&priv[0][0])[s] = 0.0;
@@ -1896,13 +1894,12 @@ int dfb::solve_data_term_ev(float *nodes, int M, const void *node_grid, const fl
     }
     const int img_cols = (flags >> 8) & 0xffff;
     const int patch_cols = (img_cols > 0 && N % img_cols == 0 && img_cols % 32 == 0 && (N / img_cols) % 8 == 0) ? img_cols : 0;
-    launch_pdl(solve_prepare_kernel, dim3(ws.prepare_blocks), dim3(256), 0, s, nodes, M, node_grid, canon, live, N, stride, ws, patch_cols, knn_warp_list_enabled());
+    launch_pdl(solve_prepare_kernel, dim3(ws.prepare_blocks), dim3(256), 0, s, nodes, M, node_grid, canon, live, N, stride, ws, patch_cols);
     DF_LAUNCH_CHECK();
     launch_pdl(solve_blockscan_kernel, dim3(div_up(M, 8)), dim3(256), 0, s, ws, M);
     DF_LAUNCH_CHECK();
     launch_pdl(solve_scan_kernel, dim3(1), dim3(1024), 0, s, ws, M);
     DF_LAUNCH_CHECK();
-    static const int lpt = [] { const char *e = getenv("DF_SOLVE_LPT"); return e ? atoi(e) : 1; }();    // A/B: heaviest rows first
     // image-shaped vertices: tile records (DF_SOLVE_TILES=0 disables), with the per-entry kernels behind them as the fallback
     static const int want_tiles = [] { const char *e = getenv("DF_SOLVE_TILES"); return e ? atoi(e) : 1; }();
     const int cols = (flags >> 8) & 0xffff;
@@ -1910,12 +1907,12 @@ int dfb::solve_data_term_ev(float *nodes, int M, const void *node_grid, const fl
     if (tiles) {
         launch_pdl(solve_tiles_kernel, dim3(ws.ntiles), dim3(TILE_PIX), 0, s, ws, cols, N / cols);
         DF_LAUNCH_CHECK();
-        launch_pdl(solve_rows_tiles_kernel, dim3(M), dim3(RT_THREADS), 0, s, ws, M, N, flags & DF_SOLVE_REF_GRAPH_QUIRK, lpt);
+        launch_pdl(solve_rows_tiles_kernel, dim3(M), dim3(RT_THREADS), 0, s, ws, M, N, flags & DF_SOLVE_REF_GRAPH_QUIRK);
         DF_LAUNCH_CHECK();
     }
     launch_pdl(solve_fill_kernel, dim3(ws.prepare_blocks), dim3(256), 0, s, ws, N, tiles ? 1 : 0, patch_cols);
     DF_LAUNCH_CHECK();
-    launch_pdl(solve_rows_kernel, dim3(M), dim3(ROWS_THREADS), 0, s, ws, M, N, flags & DF_SOLVE_REF_GRAPH_QUIRK, lpt, tiles ? 1 : 0);
+    launch_pdl(solve_rows_kernel, dim3(M), dim3(ROWS_THREADS), 0, s, ws, M, N, flags & DF_SOLVE_REF_GRAPH_QUIRK, tiles ? 1 : 0);
     DF_LAUNCH_CHECK();
     if (before_lm && cudaEventRecord(before_lm, s) != cudaSuccess) return (int)cudaGetLastError();
     // One cluster when the system fits its shared memory (16 CTAs = the non-portable maximum: half the rows, hence half the mat-vec

@@ -5,7 +5,6 @@
 // in shared memory and every thread scans them for its own point.
 #include "warp_common.cuh"
 #include "volscan.cuh"
-#include <cstdlib>
 
 using namespace dfb;
 
@@ -13,11 +12,10 @@ namespace {
 
 __global__ void __launch_bounds__(256) knn8_kernel(const float *__restrict__ nodes, int M, const void *__restrict__ grid,
                                                    const float *__restrict__ queries, int N,
-                                                   int qstride, int *__restrict__ idx, float *__restrict__ d2, int warp_list)
+                                                   int qstride, int *__restrict__ idx, float *__restrict__ d2)
 {
     DF_PDL_ENTRY();
     __shared__ KnnSmem sm;
-    __shared__ float4 knn_wl[8][KNN_WL_CAP];
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
     float qx = 0.f, qy = 0.f, qz = 0.f;
     bool valid = false;
@@ -27,8 +25,7 @@ __global__ void __launch_bounds__(256) knn8_kernel(const float *__restrict__ nod
         valid = !(isnan(qx) || isnan(qy) || isnan(qz));
     }
     int bi[8]; float bd[8];
-    if (grid && warp_list) knn8_grid_warp(grid, valid, qx, qy, qz, knn_wl[threadIdx.x >> 5], bi, bd);
-    else if (grid) knn8_grid(grid, valid, qx, qy, qz, bi, bd);
+    if (grid) knn8_grid(grid, valid, qx, qy, qz, bi, bd);
     else knn8_scan(nodes, M, valid, qx, qy, qz, sm, bi, bd);
     if (q < N) {
 #pragma unroll
@@ -43,7 +40,6 @@ struct WarpParams {
     int flags;
     int *idx; float *w;       // neighbours / weights: outputs, or inputs when DF_WARP_REUSE_KNN
     int cols;                 // > 0: the points are an image of that many columns (DF_WARP_IMAGE_COLS): warps take 8 x 4 pixel patches
-    int warp_list;            // warp-cooperative candidate lists for the 8-NN (DF_KNN_WARP_LIST, default on)
 };
 
 // cv::Affine3f * Vec3f (opencv2/core/affine.hpp): m0*x + m1*y + m2*z + m3 evaluated left to right
@@ -62,7 +58,6 @@ __global__ void __launch_bounds__(256) warp_kernel(const WarpParams p)
 {
     DF_PDL_ENTRY();
     __shared__ KnnSmem sm;
-    __shared__ float4 knn_wl[kReuse ? 1 : 8][kReuse ? 1 : KNN_WL_CAP];
     const int q = kReuse ? (int)(blockIdx.x * blockDim.x + threadIdx.x) : patch_vertex(blockIdx.x, threadIdx.x, p.cols);
     float3 pt = make_float3(0.f, 0.f, 0.f), nr = pt;
     bool valid = false;
@@ -87,8 +82,7 @@ __global__ void __launch_bounds__(256) warp_kernel(const WarpParams p)
         for (int i = 0; i < 8; ++i) bd[i] = 0.f;
         valid = valid && bi[0] >= 0;          // rows the earlier pass skipped (NaN) carry idx = -1
     } else {
-        if (p.grid && p.warp_list) knn8_grid_warp(p.grid, valid, pt.x, pt.y, pt.z, knn_wl[threadIdx.x >> 5], bi, bd);
-        else if (p.grid) knn8_grid(p.grid, valid, pt.x, pt.y, pt.z, bi, bd);
+        if (p.grid) knn8_grid(p.grid, valid, pt.x, pt.y, pt.z, bi, bd);
         else knn8_scan(p.nodes, p.M, valid, pt.x, pt.y, pt.z, sm, bi, bd);
         if (q >= p.N) return;
     }
@@ -185,17 +179,11 @@ __global__ void __launch_bounds__(256) warp_cursor_kernel(const WarpParams p, co
 
 }  // namespace
 
-int dfb::knn_warp_list_enabled()
-{
-    static const int on = [] { const char *e = getenv("DF_KNN_WARP_LIST"); return e ? atoi(e) : 0; }();
-    return on;
-}
-
 extern "C" int df_knn8(const float *nodes, int M, const void *node_grid, const float *queries, int N, int qstride, int32_t *idx, float *d2,
                        void *stream)
 {
     if (N <= 0) return 0;
-    launch_pdl(knn8_kernel, dim3(div_up(N, 256)), dim3(256), 0, (cudaStream_t)stream, nodes, M, node_grid, queries, N, qstride, idx, d2, knn_warp_list_enabled());
+    launch_pdl(knn8_kernel, dim3(div_up(N, 256)), dim3(256), 0, (cudaStream_t)stream, nodes, M, node_grid, queries, N, qstride, idx, d2);
     DF_LAUNCH_CHECK();
     return 0;
 }
@@ -216,7 +204,7 @@ extern "C" int df_warp(const float *nodes, int M, const void *node_grid, float *
         if (e != cudaSuccess) { cudaFreeAsync(scratch, s); return (int)e; }
         WarpParams p;
         p.nodes = nodes; p.M = M; p.grid = node_grid; p.points = points; p.normals = normals; p.N = N; p.stride = stride;
-        p.w2l = make_aff(warp_to_live); p.flags = flags; p.idx = nullptr; p.w = nullptr; p.cols = 0; p.warp_list = 0;
+        p.w2l = make_aff(warp_to_live); p.flags = flags; p.idx = nullptr; p.w = nullptr; p.cols = 0;
         launch_pdl(warp_cursor_count_kernel, dim3(nblocks), dim3(256), 0, s, (const float *)points, (const float *)normals, N, stride, scratch, scratch + nblocks);
         launch_pdl(warp_cursor_scan_kernel, dim3(1), dim3(1024), 0, s, scratch, nblocks);
         launch_pdl(warp_cursor_kernel, dim3(nblocks), dim3(256), 0, s, p, (const int *)scratch, (const int *)(scratch + nblocks));
@@ -230,7 +218,6 @@ extern "C" int df_warp(const float *nodes, int M, const void *node_grid, float *
     p.w2l = make_aff(warp_to_live); p.flags = flags; p.idx = idx; p.w = w;
     const int cols = (flags >> 8) & 0xffff;                      // DF_WARP_IMAGE_COLS: 8 x 4 pixel patches per warp when the shape allows it
     p.cols = (cols > 0 && N % cols == 0 && cols % 32 == 0 && (N / cols) % 8 == 0) ? cols : 0;
-    p.warp_list = knn_warp_list_enabled();
     if (flags & DF_WARP_REUSE_KNN) launch_pdl(warp_kernel<true>, dim3(div_up(N, 256)), dim3(256), 0, (cudaStream_t)stream, p);
     else launch_pdl(warp_kernel<false>, dim3(div_up(N, 256)), dim3(256), 0, (cudaStream_t)stream, p);
     DF_LAUNCH_CHECK();

@@ -262,29 +262,6 @@ __device__ __forceinline__ bool knn8_bvh_greedy_seed(const float4 *__restrict__ 
     return full;
 }
 
-// A cheap upper bound on the 8th-nearest distance for knn8_bvh_bounded when no neighbouring result is at hand: descend to the leaf
-// whose boxes are nearest at every level (no backtracking) and take the largest distance to its eight nodes.  Any eight distinct
-// nodes bound the 8th-nearest distance; a padded leaf (fewer than eight nodes) yields FLT_MAX, i.e. an unbounded search.
-__device__ __forceinline__ float knn8_bvh_greedy_bound(const float4 *__restrict__ box, const float4 *__restrict__ leaf, int L, float qx, float qy, float qz)
-{
-    int i = 0;
-    while (i < L - 1) {
-        const int a = 2 * i + 1, b = a + 1;
-        const float da = bvh_box_dist2(__ldg(box + 2 * a), __ldg(box + 2 * a + 1), qx, qy, qz);
-        const float db = bvh_box_dist2(__ldg(box + 2 * b), __ldg(box + 2 * b + 1), qx, qy, qz);
-        i = da <= db ? a : b;
-    }
-    const float4 *e = leaf + (size_t)(i - (L - 1)) * NODEGRID_BVH_LEAF;
-    float limit = 0.f;
-#pragma unroll
-    for (int k = 0; k < NODEGRID_BVH_LEAF; ++k) {
-        const float4 nd = __ldg(e + k);
-        const float d0 = qx - nd.x, d1 = qy - nd.y, d2 = qz - nd.z;
-        limit = fmaxf(limit, d0 * d0 + d1 * d1 + d2 * d2);
-    }
-    return limit < 3.402823466e+38f ? limit : 3.402823466e+38f;      // inf (padding) or NaN -> unbounded
-}
-
 __device__ __forceinline__ void knn8_grid(const void *__restrict__ grid, bool valid, float qx, float qy, float qz, int (&bi)[8], float (&bd)[8])
 {
 #pragma unroll
@@ -374,127 +351,9 @@ __device__ __forceinline__ void knn8_grid(const void *__restrict__ grid, bool va
     for (int i = 0; i < 8; ++i) if (bi[i] == 0x7fffffff) bi[i] = -1;
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// Warp-cooperative 8-NN (round 2, second session).  The 32 queries of a warp are neighbours in the image (an 8 x 4 pixel patch, or 32
-// consecutive vertices), so their neighbour sets overlap almost completely and a small superset is cheap to certify: with c the centroid
-// of the warp's valid queries, h >= |x - c| for each of them and R >= d8(c) (distance from c to its 8th nearest node), every query x has
-// d8(x) <= R + h (the eight nodes nearest to c are that close to x), hence each of its eight nearest nodes n has |n - c| <= |n - x| + h
-// <= R + 2h.  The warp scans the grid cells around c together (lane-strided over the contiguous node runs of the grid rows): pass A forms R
-// as the 8th smallest of the 32 lane minima (distances of distinct nodes, so >= d8(c)), pass B compacts the nodes within (R + 2h)(1 + 2e-4)
-// of c into shared memory (ballot ranks), and every lane then ranks those ~20-60 candidates (broadcast reads) with the float distance and the
-// (distance, index) order of every other search path: the result IS knn8_grid's, at a fraction of the divergent per-lane cell walk
-// (12-17 of 32 lanes active, DESIGN 3.1).  Warps whose queries are far from the nodes or spread out (depth edges: large h) get no list
-// -- fewer than eight nodes within three cells of c, more than KNN_WL_CAP candidates or more than KNN_WL_ROWS grid rows -- and fall
-// back to knn8_grid lane by lane.  ALL 32 lanes of the warp must call this.
-// Measured in the frame loop: bit-exact, but no faster than the lane-by-lane walk once a warp's queries are an
-// 8 x 4 pixel patch -- the two cooperative passes are chains of dependent row-bound
-// loads of their own.  What DID pay is the patch mapping itself (patch_vertex below: tighter
-// queries walk the same cells).  The lists are therefore opt-in (DF_KNN_WARP_LIST=1), the patch mapping is the default.
-constexpr int KNN_WL_CAP = 96;        // candidates per warp: 1.5 KB of float4 (x, y, z, index bits)
-constexpr int KNN_WL_ROWS = 49;       // grid rows (fixed y, z) pass B may touch
-
-__device__ __forceinline__ void knn8_grid_warp(const void *__restrict__ grid, bool valid, float qx, float qy, float qz, float4 *__restrict__ wl,
-                                               int (&bi)[8], float (&bd)[8])
-{
-    const unsigned full = 0xffffffffu;
-    const int lane = threadIdx.x & 31;
-    const unsigned vmask = __ballot_sync(full, valid);
-    int K = -1;                                                    // candidates in wl; -1: no list
-    if (vmask) {                                                   // (warp-uniform)
-        const NodeGridHeader h = *reinterpret_cast<const NodeGridHeader *>(grid);
-        const int *cell_start = nodegrid_cell_start(grid);
-        const float4 *sorted = nodegrid_sorted(grid, h.ncell);
-        float sx = valid ? qx : 0.f, sy = valid ? qy : 0.f, sz = valid ? qz : 0.f;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { sx += __shfl_xor_sync(full, sx, o); sy += __shfl_xor_sync(full, sy, o); sz += __shfl_xor_sync(full, sz, o); }
-        const float inv_n = 1.f / (float)__popc(vmask);
-        const float cx = sx * inv_n, cy = sy * inv_n, cz = sz * inv_n;       // any point works as the centre: h is measured from it
-        float hh = 0.f;
-        if (valid) { const float a = qx - cx, b = qy - cy, c = qz - cz; hh = a * a + b * b + c * c; }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) hh = fmaxf(hh, __shfl_xor_sync(full, hh, o));
-        const float hr = sqrtf(hh) * 1.00001f;
-        if (cx == cx && cy == cy && cz == cz && hr < 3.0e37f) {
-            const int ccx = min(max((int)floorf((cx - h.ox) * h.inv_cell), 0), h.gx - 1);
-            const int ccy = min(max((int)floorf((cy - h.oy) * h.inv_cell), 0), h.gy - 1);
-            const int ccz = min(max((int)floorf((cz - h.oz) * h.inv_cell), 0), h.gz - 1);
-            // pass A: lane minima over the cells within Chebyshev distance r of c's cell (every node is visited by exactly one lane)
-            float m = 3.402823466e+38f;
-            int have = 0;
-            for (int r = 1; r <= 3 && have < 8; ++r) {
-                m = 3.402823466e+38f;
-                for (int z = max(ccz - r, 0); z <= min(ccz + r, h.gz - 1); ++z)
-                    for (int y = max(ccy - r, 0); y <= min(ccy + r, h.gy - 1); ++y) {
-                        const int row = h.gx * (y + h.gy * z);
-                        const int b = __ldg(cell_start + row + max(ccx - r, 0)), e = __ldg(cell_start + row + min(ccx + r, h.gx - 1) + 1);
-                        for (int it = b + lane; it < e; it += 32) {
-                            const float4 nd = __ldg(sorted + it);
-                            const float d0 = cx - nd.x, d1 = cy - nd.y, d2 = cz - nd.z;
-                            m = fminf(m, d0 * d0 + d1 * d1 + d2 * d2);        // (a NaN node never lowers the minimum)
-                        }
-                    }
-                have = __popc(__ballot_sync(full, m < 3.0e38f));
-            }
-            if (have >= 8) {
-                float R2 = 0.f;
-                for (int k = 0; k < 8; ++k) {                      // 8th smallest lane minimum: distances of eight distinct nodes
-                    float t = m;
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) t = fminf(t, __shfl_xor_sync(full, t, o));
-                    R2 = t;
-                    const unsigned holders = __ballot_sync(full, m == t);
-                    if (lane == __ffs(holders) - 1) m = 3.402823466e+38f;
-                }
-                const float rho = (sqrtf(R2) * 1.00001f + 2.f * hr) * 1.0002f + h.cell * 1e-4f;
-                const float rho2 = rho * rho;
-                const int x0 = max((int)floorf((cx - rho - h.ox) * h.inv_cell), 0), x1 = min((int)floorf((cx + rho - h.ox) * h.inv_cell), h.gx - 1);
-                const int y0 = max((int)floorf((cy - rho - h.oy) * h.inv_cell), 0), y1 = min((int)floorf((cy + rho - h.oy) * h.inv_cell), h.gy - 1);
-                const int z0 = max((int)floorf((cz - rho - h.oz) * h.inv_cell), 0), z1 = min((int)floorf((cz + rho - h.oz) * h.inv_cell), h.gz - 1);
-                if (x0 <= x1 && y0 <= y1 && z0 <= z1 && (y1 - y0 + 1) * (z1 - z0 + 1) <= KNN_WL_ROWS && rho < 3.0e18f) {
-                    // pass B: the nodes within rho of c, compacted in visiting order (a function of the data only)
-                    K = 0;
-                    for (int z = z0; z <= z1; ++z)
-                        for (int y = y0; y <= y1; ++y) {
-                            const int row = h.gx * (y + h.gy * z);
-                            const int b = __ldg(cell_start + row + x0), e = __ldg(cell_start + row + x1 + 1);
-                            for (int it0 = b; it0 < e; it0 += 32) {
-                                const int it = it0 + lane;
-                                float4 nd = make_float4(0.f, 0.f, 0.f, 0.f);
-                                bool in = false;
-                                if (it < e) {
-                                    nd = __ldg(sorted + it);
-                                    const float d0 = cx - nd.x, d1 = cy - nd.y, d2 = cz - nd.z;
-                                    in = d0 * d0 + d1 * d1 + d2 * d2 <= rho2;
-                                }
-                                const unsigned mk = __ballot_sync(full, in);
-                                if (in) { const int pos = K + __popc(mk & ((1u << lane) - 1u)); if (pos < KNN_WL_CAP) wl[pos] = nd; }
-                                K += __popc(mk);
-                            }
-                        }
-                    if (K > KNN_WL_CAP) K = -1;
-                }
-            }
-        }
-    }
-    __syncwarp();
-    if (K < 0) { knn8_grid(grid, valid, qx, qy, qz, bi, bd); return; }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { bi[i] = 0x7fffffff; bd[i] = 3.402823466e+38f; }
-    if (valid) {
-#pragma unroll 4
-        for (int k = 0; k < K; ++k) {
-            const float4 nd = wl[k];
-            const float d0 = qx - nd.x, d1 = qy - nd.y, d2 = qz - nd.z;
-            knn8_insert_lex(bi, bd, d0 * d0 + d1 * d1 + d2 * d2, __float_as_int(nd.w));
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) if (bi[i] == 0x7fffffff) bi[i] = -1;
-    __syncwarp();                                                  // the list may be rebuilt by the caller's next search
-}
-
 // Vertex handled by thread `tid` of 256-thread block `blk`: 256 consecutive vertices, or -- for an image of `cols` columns (cols % 32 == 0,
-// rows % 8 == 0) -- a 32 x 8 pixel region whose warps are 8 x 4 patches (the tighter a warp's queries, the shorter its candidate list).
+// rows % 8 == 0) -- a 32 x 8 pixel region whose warps are 8 x 4 patches.  Measured in the frame loop: the patch mapping pays because a warp's
+// tighter queries walk the same grid cells in knn8_grid; warp-cooperative candidate lists on top of it were bit-exact but no faster.
 __device__ __forceinline__ int patch_vertex(int blk, int tid, int cols)
 {
     if (cols <= 0) return blk * 256 + tid;
@@ -549,14 +408,12 @@ __device__ __forceinline__ float3 qrotate(const Quat q, const float3 v)
     const float3 c = cross3(scale3(qv, 2.f), inner);
     return make_float3(v.x + c.x, v.y + c.y, v.z + c.z);
 }
-// WarpField::weighting, warp_field.cpp:238-241: double exp of a float argument, narrowed to float
 // WarpField::weighting (warp_field.cpp:262-265): (float)exp((double)x), x = -d2 / (2 w^2) in float.  The generic double exp is ~60 instructions and
 // was a large share of the warped-fusion kernel.  With the reference's node weight (3, i.e. sigma = 3 m) x
 // lies in [-0.06, 0]; for x in [-0.5, 0] the value is formed as exp(-1/4) * P13(x + 1/4), a degree-13 Taylor polynomial in fused double
 // arithmetic (truncation 2.4e-18, |r| <= 1/4): after the rounding to float it equals (float)exp((double)x) of a correctly rounded libm for
 // EVERY float in the interval -- checked exhaustively, 1,056,964,609 values, by tests/test_weight_exp.py against glibc (the oracle's exp).
 // Anything else (other node weights, NaN) takes the generic path.
-__device__ __forceinline__ float node_weighting_generic(float d2, float node_w) { return (float)exp((double)(-d2 / (2 * node_w * node_w))); }
 // out of line: the generic exp is ~60 instructions, and kernels that weight eight neighbours per element would carry eight copies of it next to
 // the polynomial -- the warped-fusion kernel turned out to be bound by instruction fetch
 static __device__ __noinline__ float node_weighting_slow(float x) { return (float)exp((double)x); }

@@ -356,11 +356,11 @@ def test_solve_row_overflow_is_loud_and_leaves_the_field_unchanged():
 
 
 @pytest.mark.parametrize("env", [{"DF_SOLVE_LM_IMPL": "5", "DF_SOLVE_MERGED": "0"}, {"DF_SOLVE_LM_IMPL": "5", "DF_SOLVE_BALANCED": "0"},
-                                 {"DF_SOLVE_V6_FORCE_FALLBACK": "1"}, {"DF_SOLVE_LM_IMPL": "1"}, {"DF_SOLVE_LM_CTAS": "8"}, {"DF_KNN_WARP_LIST": "1"}])
+                                 {"DF_SOLVE_V6_FORCE_FALLBACK": "1"}, {"DF_SOLVE_LM_IMPL": "1"}, {"DF_SOLVE_LM_CTAS": "8"}])
 def test_alternative_icp_and_solve_kernels_in_subprocess(env):
     """The variants that are selected once per process: the v5 cluster LM
     (two exchanges per PCG step) with two reductions per step / fixed lanes per row, v5 as the fallback the default v6 kernel hands a frame
-    to when its halo tables do not fit, the one-block LM fallback, the 8-CTA cluster and the warp-cooperative candidate lists of the 8-NN.  Each re-runs this file's ICP / solve parity tests under
+    to when its halo tables do not fit, the one-block LM fallback and the 8-CTA cluster.  Each re-runs this file's ICP / solve parity tests under
     the switch in a fresh interpreter."""
     import os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -429,12 +429,12 @@ def test_solve_tile_assembly_matches_per_entry_path_and_oracle(orc, coherent):
 
 
 @pytest.mark.parametrize("cols,rows", [(256, 160), (200, 100)])
-def test_knn_warp_lists_on_image_shaped_queries(orc, cols, rows):
-    """The warp-cooperative candidate lists of the 8-NN (knn8_grid_warp): queries that are neighbours in the image -- the case the lists are
-    built for, which the random point sets of test_knn_and_warp never produce -- against the oracle's exhaustive search: indices and squared
-    distances bit for bit, through df_knn8 (32 consecutive queries per warp) and through df_warp's neighbour output with the 8 x 4 patch
-    mapping of DF_WARP_IMAGE_COLS (256 x 160; 200 x 100 does not qualify and keeps the linear map).  Includes duplicated nodes (ties at
-    every rank), NaN pixels, a depth edge (a warp whose queries straddle two surfaces) and a far region (no list: lane-by-lane fallback)."""
+def test_knn_on_image_shaped_queries(orc, cols, rows):
+    """The 8-NN grid walk (knn8_grid) on queries that are neighbours in the image, which the random point sets of test_knn_and_warp never
+    produce, against the oracle's exhaustive search: indices and squared distances bit for bit, through df_knn8 (32 consecutive queries per
+    warp) and through df_warp's neighbour output with the 8 x 4 patch mapping of DF_WARP_IMAGE_COLS (256 x 160; 200 x 100 does not qualify
+    and keeps the linear map).  Includes duplicated nodes (ties at every rank), NaN pixels, a depth edge (a warp whose queries straddle two
+    surfaces) and a far region 0.6 m off the node cloud."""
     rng = np.random.default_rng(cols)
     N = cols * rows
     u, v = np.meshgrid(np.linspace(-0.3, 0.3, cols), np.linspace(-0.2, 0.2, rows))

@@ -5,8 +5,6 @@ change a bit.  Per case the largest |GPU - f64| / bar, the ambiguous fractions, 
 import hashlib
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
@@ -268,20 +266,3 @@ def test_integrate_warped_against_oracle_and_float64(orc, cid):
     report["wall_s"] = round(time.time() - t0, 1)
     _print(cid, report)
 
-
-def output_digests():
-    """the digest of every case's volumes, activity maps and counts"""
-    import oracle.orc as orc
-    return {cid: Run(wc.case(cid), wc.case_nodes(orc, wc.case(cid))).digest() for cid in wc.CASES}
-
-
-def test_min_blocks_3_in_subprocess():
-    """DF_FUSION_MIN_BLOCKS is read once per process: the kMinBlocks = 3 instances store what the default ones store, on every case"""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = "import sys, json; sys.path[:0] = ['tests', '.']; import test_warp_reference_gpu as t; print(json.dumps(t.output_digests()))"
-    out = []
-    for env in ({}, {"DF_FUSION_MIN_BLOCKS": "3"}):
-        r = subprocess.run([sys.executable, "-c", code], cwd=root, env=dict(os.environ, **env), capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, r.stderr[-3000:]
-        out.append(json.loads(r.stdout.strip().splitlines()[-1]))
-    assert out[0] == out[1]
