@@ -59,6 +59,31 @@ class KinfuParams(C.Structure):
                 ("fusion_weight_scale", C.c_float), ("extend_radius", C.c_float)]
 
 
+class RelocGate(C.Structure):
+    """df_reloc_gate (include/dfusion.h): the ICP's T and ok and the gate's counts"""
+    _fields_ = [("T", C.c_float * 12), ("ok", C.c_int), ("n_valid", C.c_int), ("n_in", C.c_int), ("pad", C.c_int), ("sum_sq", C.c_double)]
+
+
+# include/dfusion.h DF_RELOC_*: the relocaliser's constants
+RELOC_FERNS = 500
+RELOC_CANDIDATES = 3
+RELOC_KEYFRAMES = 512
+RELOC_NEAR_MM = 400
+RELOC_FAR_MM = 3000
+RELOC_SEED = 0x5eedf00d
+RELOC_HARVEST_FERNS = 40
+RELOC_MIN_VALID = 5000
+RELOC_MIN_INLIER_FRAC = 0.1
+RELOC_MAX_RMS = 0.03
+RELOC_GATE_WS_BYTES = 4096
+
+
+class RelocMatch(C.Structure):
+    """df_reloc_match (include/dfusion.h): the lookup's candidates, the append and the database's count"""
+    _fields_ = [("index", C.c_int * RELOC_CANDIDATES), ("dissimilarity", C.c_int * RELOC_CANDIDATES), ("appended", C.c_int), ("count", C.c_int),
+                ("pose", (C.c_float * 12) * RELOC_CANDIDATES)]
+
+
 class F2Params(C.Structure):
     """df_f2_params (include/dfusion.h)"""
     _fields_ = [("reg_lambda", C.c_double), ("tukey_c", C.c_double), ("huber_delta", C.c_double), ("lm_mu", C.c_double),
@@ -190,6 +215,12 @@ PROTOTYPES = {
     "df_icp_estimate_color": (_i, [C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_sz),
                                    C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_i), C.POINTER(_i), C.POINTER(_sz), _i, C.POINTER(_i), Intr, _f,
                                    _f, _f, _f, _vp, _vp, _vp, _vp]),
+    "df_reloc_fern_table": (_i, [C.c_ulonglong, _i, _i, _i, _vp]),
+    "df_fern_encode": (_i, [_vp, _sz, _i, _i, _vp, _i, _vp, _vp]),
+    "df_fern_match": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, Aff3f, _vp, _vp]),
+    "df_icp_inliers": (_i, [_vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz, _i, _i, Intr, _vp, _vp, _f, _f, _vp, _vp, _vp]),
+    "df_reloc_gate_accepts": (_i, [C.POINTER(RelocGate)]),
+    "df_kinfu_get_keyframes": (_i, [_vp, _vp, _vp, _i, C.POINTER(_i)]),
 }
 
 # include/dfusion.h DF_COLOR_TRACK_WEIGHT / DF_COLOR_TRACK_MAX_RESIDUAL: the frame loop's photometric weight and residual gate

@@ -788,7 +788,8 @@ static df_kinfu_params params_to(const KinFuParams& p)
     for (int i = 0; i < 4; ++i) d.icp_iter_num[i] = i < (int)p.icp_iter_num.size() ? p.icp_iter_num[i] : 0;
     d.tsdf_min_camera_movement = p.tsdf_min_camera_movement; d.tsdf_trunc_dist = p.tsdf_trunc_dist; d.tsdf_max_weight = p.tsdf_max_weight;
     d.raycast_step_factor = p.raycast_step_factor; d.gradient_delta_factor = p.gradient_delta_factor;
-    d.flags |= p.dfusion_flags & (DF_KINFU_WARPED_INTEGRATE | DF_KINFU_EXTEND_FIELD | DF_KINFU_COLOR | DF_KINFU_COLOR_TRACKING | DF_KINFU_WARPED_COLOR);
+    d.flags |= p.dfusion_flags & (DF_KINFU_WARPED_INTEGRATE | DF_KINFU_EXTEND_FIELD | DF_KINFU_COLOR | DF_KINFU_COLOR_TRACKING | DF_KINFU_WARPED_COLOR |
+                                  DF_KINFU_RELOCALISE);
     d.fusion_weight_scale = p.fusion_weight_scale; d.extend_radius = p.extend_radius;
     return d;
 }
@@ -904,6 +905,13 @@ bool KinFu::operator()(const cuda::Depth& depth, const cuda::Image& image)
     }
     return r == 1;
 }
+bool KinFu::isLost() const
+{
+    long long info[14] = {};
+    df_kinfu_get_info(handle_, info, 14);
+    return info[13] != 0;
+}
+
 bool KinFu::save(const std::string& path) const
 {
     size_t n = 0;

@@ -94,6 +94,16 @@ struct KinFu {
     bool field_frame = false;            // the last dynamicfusion() warped and solved (a warp field, not a rigid frame)
     float lm_shift[3] = {0.f, 0.f, 0.f}; // R_vol * (vs/2): extraction puts voxel i at (i + 1/2) vs, integrate and the ray-cast at i vs
     long long lm_fallbacks = 0; bool lm_fell_back = false;   // frames without a live model; info[12]
+    // DF_KINFU_RELOCALISE (all allocated with the flag only): the fern table of the level-2 image, the frame's code, the keyframe database
+    // (codes, poses, count on the device: the match kernel appends without a host round trip), the gate's workspace and result with its
+    // pinned copy, the lookup's result, and the pyramid a keyframe candidate is ray-cast into (the kept previous-frame maps survive a
+    // failed attempt).  lost: the last frame failed the gate; the last good pose is poses.back().  info[13..16]
+    DevMem<int32_t> fern_table; DevMem<uint8_t> frame_code, kf_codes; DevMem<float> kf_poses; DevMem<int> kf_count;
+    DevMem<void> gate_ws; DevMem<df_reloc_gate> gate; DevMem<df_reloc_match> match;
+    df_reloc_gate *gate_host = nullptr; df_reloc_match *match_host = nullptr;
+    Img rl_pts[MAX_LEVELS], rl_nrm[MAX_LEVELS];
+    bool lost = false;
+    long long lost_frames = 0, relocalisations = 0;
     float *pinned = nullptr;            // 16 floats: T(12) + ok
     std::vector<float> poses;            // 12 floats per pose
     int frame_counter = 0, resets = 0, last_ok = 1, launches = 0;
@@ -128,6 +138,8 @@ struct KinFu {
         for (cudaEvent_t e : {ev_volume_ready, ev_before_lm, ev_extract_done}) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
         cudaFreeHost(pinned);
+        if (gate_host) cudaFreeHost(gate_host);
+        if (match_host) cudaFreeHost(match_host);
     }
 };
 
@@ -168,6 +180,7 @@ inline df_volume vol_of(const KinFu &k)
 }
 
 inline bool color_on(const KinFu &k) { return (k.p.flags & DF_KINFU_COLOR) != 0; }
+inline bool reloc_on(const KinFu &k) { return (k.p.flags & DF_KINFU_RELOCALISE) != 0; }
 // the colour volume as a df_volume, for the calls that treat it as one (clear, brick packing)
 inline df_volume color_vol_of(const KinFu &k) { df_volume v = vol_of(k); v.data = k.color_vol; return v; }
 

@@ -10,7 +10,7 @@ namespace {
 
 constexpr char SNAP_MAGIC[8] = {'D', 'F', 'U', 'S', 'N', 'A', 'P', '\0'};
 // version 1; version 2 (objects with DF_KINFU_COLOR) appends the colour sections; version 3 (a colour camera set) then its calibration;
-// version 4 (a lens set) any of those, then the lens section
+// version 4 (a lens set) any of those, then the lens section; version 5 (DF_KINFU_RELOCALISE) any of those, then the relocaliser section
 uint32_t snap_version(const df_kinfu_params &p, bool camera, bool lenses)
 {
     return lenses ? 4u : (p.flags & DF_KINFU_COLOR) ? (camera ? 3u : 2u) : 1u;
@@ -29,7 +29,16 @@ struct SnapCounters {
     int64_t solve_overflows;
     uint64_t payload_bytes;
 };
-static_assert(sizeof(SnapHeader) == 32 && sizeof(SnapCounters) == 40, "snapshot sections are packed");
+// the head of the version-5 relocaliser section; then count x n_ferns code bytes, count x 12 pose floats, and the u64 section length
+struct RelocSection {
+    uint32_t base_version;                 // the version (1-4) the rest of the snapshot has
+    uint8_t lost, pad[3];
+    int64_t lost_frames, relocalisations;
+    uint64_t seed;
+    int32_t count, n_ferns;
+};
+static_assert(sizeof(SnapHeader) == 32 && sizeof(SnapCounters) == 40 && sizeof(RelocSection) == 40, "snapshot sections are packed");
+size_t reloc_section_bytes(int count) { return sizeof(RelocSection) + (size_t)count * (DF_RELOC_FERNS + 48) + 8; }
 
 // sum over the little-endian u64 words w_i of the (zero-padded) body of splitmix64(w_i ^ i * golden), plus the length
 uint64_t snap_checksum(const unsigned char *p, size_t n)
@@ -62,6 +71,10 @@ struct SnapLayout {
     // version 4: the lens section at `lenses`
     bool has_lenses = false;
     size_t lenses = 0;
+    // version 5: the relocaliser section at `reloc`
+    bool has_reloc = false;
+    RelocSection r = {};
+    size_t reloc = 0;
 };
 
 df_volume geometry_of(const df_kinfu_params &p)
@@ -105,6 +118,7 @@ void layout_sections(SnapLayout &L)
     }
     if (L.has_camera) { L.camera = o; o += sizeof(df_color_camera); }
     if (L.has_lenses) { L.lenses = o; o += LENS_SECTION; }
+    if (L.has_reloc) { L.reloc = o; o += reloc_section_bytes(L.r.count); }
     L.total = o;
 }
 
@@ -123,7 +137,7 @@ int parse_snapshot(const void *buf, size_t bytes, SnapLayout &L)
     SnapHeader h;
     memcpy(&h, b, sizeof h);
     if (memcmp(h.magic, SNAP_MAGIC, 8) != 0) return reject("not a snapshot (magic)");
-    if (h.version < 1 || h.version > 4) return reject("unsupported format version");
+    if (h.version < 1 || h.version > 5) return reject("unsupported format version");
     if (h.header_bytes != sizeof(SnapHeader)) return reject("header length");
     if (h.total_bytes != bytes) return reject("length differs from the header's (truncated or padded)");
     if (bytes < fixed) return reject("shorter than its fixed sections");
@@ -134,6 +148,25 @@ int parse_snapshot(const void *buf, size_t bytes, SnapLayout &L)
     memcpy(&L.c, b + o, sizeof L.c);
     const SnapCounters &c = L.c;
     const df_kinfu_params &p = L.p;
+    // version 5: the relocaliser section ends the snapshot and its last 8 bytes give its length; the rest is a snapshot of its base version
+    uint32_t version = h.version;
+    L.has_reloc = version == 5;
+    if (L.has_reloc) {
+        uint64_t len = 0;
+        if (bytes < fixed + reloc_section_bytes(0)) return reject("relocaliser section lengths (truncated)");
+        memcpy(&len, b + bytes - 8, 8);
+        if (len < reloc_section_bytes(0) || len > bytes - fixed) return reject("relocaliser section lengths");
+        memcpy(&L.r, b + bytes - len, sizeof L.r);
+        const RelocSection &r = L.r;
+        if (r.base_version < 1 || r.base_version > 4) return reject("relocaliser section: base version");
+        if (r.count < 0 || r.count > DF_RELOC_KEYFRAMES) return reject("relocaliser section: more keyframes than the database holds");
+        if (r.n_ferns != DF_RELOC_FERNS || r.seed != DF_RELOC_SEED) return reject("relocaliser section: fern table differs from this library's");
+        if (r.lost > 1 || r.pad[0] || r.pad[1] || r.pad[2] || r.lost_frames < 0 || r.relocalisations < 0) return reject("relocaliser section: counters");
+        if (len != reloc_section_bytes(r.count)) return reject("relocaliser section lengths");
+        version = r.base_version;
+        bytes -= len;                                                  // the checks below see the base snapshot
+    }
+    if (L.has_reloc != ((p.flags & DF_KINFU_RELOCALISE) != 0)) return reject("relocaliser section does not match the DF_KINFU_RELOCALISE flag of its parameters");
     if (p.volume_dims[0] <= 0 || p.volume_dims[0] % 32 || p.volume_dims[1] <= 0 || p.volume_dims[2] <= 0 || p.cols <= 0 || p.rows <= 0 ||
         p.cloud_capacity < 0)
         return reject("parameters");
@@ -143,9 +176,9 @@ int parse_snapshot(const void *buf, size_t bytes, SnapLayout &L)
     if (c.payload_bytes % 4 || c.payload_bytes > 4 * (size_t)df_volume_brick_count(geometry_of(p)) * DF_BRICK * DF_BRICK * DF_BRICK ||
         (double)c.n_poses * 48 > (double)bytes || c.cloud_count > p.cloud_capacity)
         return reject("section lengths");
-    L.has_camera = h.version == 3;
-    L.has_lenses = h.version == 4;
-    if (!L.has_lenses && h.version != snap_version(p, L.has_camera, false)) return reject("format version does not match the colour flag of its parameters");
+    L.has_camera = version == 3;
+    L.has_lenses = version == 4;
+    if (!L.has_lenses && version != snap_version(p, L.has_camera, false)) return reject("format version does not match the colour flag of its parameters");
     L.color_payload_bytes = 0;
     layout_sections(L);
     if (p.flags & DF_KINFU_COLOR) {
@@ -154,9 +187,11 @@ int parse_snapshot(const void *buf, size_t bytes, SnapLayout &L)
         if (L.color_payload_bytes > bytes) return reject("colour section lengths");
         layout_sections(L);
         // version 4 of a colour object: the camera record is there when the length says so
-        if (L.has_lenses && L.total + sizeof(df_color_camera) == bytes) { L.has_camera = true; layout_sections(L); }
+        const size_t reloc_bytes = L.has_reloc ? reloc_section_bytes(L.r.count) : 0;
+        if (L.has_lenses && L.total - reloc_bytes + sizeof(df_color_camera) == bytes) { L.has_camera = true; layout_sections(L); }
     }
-    if (L.total != bytes) return reject(L.color_len ? "section lengths (colour sections included)" : "section lengths");
+    if (L.total != bytes + (L.has_reloc ? reloc_section_bytes(L.r.count) : 0))
+        return reject(L.color_len ? "section lengths (colour sections included)" : "section lengths");
     if (L.has_lenses) {
         const unsigned char *ls = b + L.lenses;
         bool any = false;
@@ -315,6 +350,13 @@ extern "C" int df_kinfu_save(void *h, void *dst_host, size_t capacity, size_t *b
     L.color_payload_bytes = col.bytes;
     L.has_camera = k->has_cam;
     L.has_lenses = k->has_depth_lens || k->has_color_lens;
+    L.has_reloc = reloc_on(*k);
+    if (L.has_reloc) {
+        int kf = 0;
+        CK(cudaMemcpy(&kf, k->kf_count, sizeof kf, cudaMemcpyDeviceToHost));
+        L.r = RelocSection{snap_version(L.p, L.has_camera, L.has_lenses), (uint8_t)k->lost, {0, 0, 0}, k->lost_frames, k->relocalisations,
+                           DF_RELOC_SEED, kf, DF_RELOC_FERNS};
+    }
     layout_sections(L);
     if (bytes_out) *bytes_out = L.total;
     if (!dst_host) return 0;
@@ -340,10 +382,19 @@ extern "C" int df_kinfu_save(void *h, void *dst_host, size_t capacity, size_t *b
         ls += 1 + sizeof(df_lens);
         ls[0] = k->has_color_lens; memcpy(ls + 1, &k->color_lens, sizeof(df_lens));
     }
+    if (L.has_reloc) {
+        unsigned char *r = b + L.reloc;
+        memcpy(r, &L.r, sizeof L.r);
+        r += sizeof L.r;
+        CK(cudaMemcpyAsync(r, k->kf_codes, (size_t)L.r.count * DF_RELOC_FERNS, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(r + (size_t)L.r.count * DF_RELOC_FERNS, k->kf_poses, (size_t)L.r.count * 48, cudaMemcpyDeviceToHost, s));
+        const uint64_t len = reloc_section_bytes(L.r.count);
+        memcpy(b + L.total - 8, &len, 8);
+    }
     CK(cudaStreamSynchronize(s));
     SnapHeader hd;
     memcpy(hd.magic, SNAP_MAGIC, 8);
-    hd.version = snap_version(L.p, L.has_camera, L.has_lenses); hd.header_bytes = sizeof hd; hd.total_bytes = L.total;
+    hd.version = L.has_reloc ? 5u : snap_version(L.p, L.has_camera, L.has_lenses); hd.header_bytes = sizeof hd; hd.total_bytes = L.total;
     hd.checksum = snap_checksum(b + sizeof hd, L.total - sizeof hd);
     memcpy(b, &hd, sizeof hd);
     return 0;
@@ -383,11 +434,18 @@ extern "C" int df_kinfu_load(void *h, const void *src_host, size_t bytes)
     }
     CK(for_each_buffer_section(*k, L, [&](void *dev, size_t off, size_t n) { return cudaMemcpyAsync(dev, b + off, n, cudaMemcpyHostToDevice, s); }));
     CK(cudaMemcpyAsync(k->cloud_count, &L.c.cloud_count, sizeof(int), cudaMemcpyHostToDevice, s));
+    if (L.has_reloc) {                                                 // the parameters match, so the object has the flag and its buffers
+        const unsigned char *r = b + L.reloc + sizeof(RelocSection);
+        CK(cudaMemcpyAsync(k->kf_codes, r, (size_t)L.r.count * DF_RELOC_FERNS, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(k->kf_poses, r + (size_t)L.r.count * DF_RELOC_FERNS, (size_t)L.r.count * 48, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(k->kf_count, &L.r.count, sizeof(int), cudaMemcpyHostToDevice, s));
+    }
     if (L.c.M > 0) CK(df_build_node_grid(k->nodes, L.c.M, k->node_grid, s));
     CK(cudaStreamSynchronize(s));
     k->f2 = L.f2;
     k->frame_counter = L.c.frame_counter; k->resets = L.c.resets; k->last_ok = L.c.last_ok; k->M = L.c.M;
     k->solve_overflows = L.c.solve_overflows;
+    if (L.has_reloc) { k->lost = L.r.lost != 0; k->lost_frames = L.r.lost_frames; k->relocalisations = L.r.relocalisations; }
     k->last_cloud = L.c.cloud_count;
     k->poses.resize((size_t)L.c.n_poses * 12);
     memcpy(k->poses.data(), b + L.poses, (size_t)L.c.n_poses * 48);

@@ -52,6 +52,16 @@ __global__ void __launch_bounds__(256) init_nodes_kernel(const float4 *cloud, in
     n[11] = 3.f;
 }
 
+// DF_KINFU_RELOCALISE, a keyframe's relocalisation: every node's transform back to init_nodes_kernel's identity; position and weight kept
+__global__ void __launch_bounds__(256) identity_transforms_kernel(int M, float *nodes)
+{
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= M) return;
+    float *n = nodes + (size_t)m * DF_NODE_STRIDE;
+    n[3] = 1.f; n[4] = 0.f; n[5] = 0.f; n[6] = 0.f;
+    n[7] = 1.f; n[8] = 0.f; n[9] = 0.f; n[10] = 0.f;
+}
+
 // order-independent 64-bit checksum of a u32 array: sum over i of mix(i, a[i]) (splitmix64 finaliser); one u64 atomicAdd per block
 __global__ void __launch_bounds__(256) digest_kernel(const uint32_t *__restrict__ a, size_t n, unsigned long long *out)
 {
@@ -122,6 +132,10 @@ int do_reset(KinFu &k)
     if (int w = wait_extract_on_main(k)) return w;
     if (k.activity && cudaMemsetAsync(k.activity, 0, k.activity_bytes, k.stream) != cudaSuccess) return (int)cudaGetLastError();
     if (color_on(k)) CK(df_clear_volume(color_vol_of(k), k.stream));
+    if (reloc_on(k)) {                                               // the keyframe database empties and a loss ends
+        k.lost = false;
+        CK(cudaMemsetAsync(k.kf_count, 0, sizeof(int), k.stream));
+    }
     return df_clear_volume(vol_of(k), k.stream);
 }
 
@@ -278,6 +292,11 @@ int preprocess(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch)
                                    out.ptr, out.pitch, s));
         k.launches += k.levels;
     }
+    if (reloc_on(k)) {                                                 // the frame's fern code, for the harvest and the lookup
+        const Img &d2 = k.cur_depth[2];
+        CK(df_fern_encode((const uint16_t *)d2.ptr, d2.pitch, d2.cols, d2.rows, k.fern_table, DF_RELOC_FERNS, k.frame_code, s));
+        ++k.launches;
+    }
     mark(k, 1);
     return 0;
 }
@@ -314,40 +333,143 @@ int first_frame(KinFu &k)
 }
 
 // ---- ICP, kinfu.cpp:268-280 (device-resident; one host read of {ok, T}), or the pose of df_kinfu_set_overrides --------
-// Appends the frame's pose.  ICP failure resets the object (kinfu.cpp:276-277), which leaves frame_counter at 0.
-int track(KinFu &k, double &t_sync0, double &t_sync1)
+// the ICP of the current pyramid against the previous-frame maps, into icp_T / icp_ok (no host read)
+int launch_icp(KinFu &k)
 {
     const df_kinfu_params &p = k.p;
     cudaStream_t s = k.stream;
+    const Levels<float> vc(k.cur_pts, k.levels), nc(k.cur_nrm, k.levels), vp(k.prev_pts, k.levels), np(k.prev_nrm, k.levels);
+    if (p.flags & DF_KINFU_USE_DEPTH) {                                // estimateTransform(depth pyramids), kinfu.cpp:271
+        const Levels<unsigned short> dc(k.cur_depth, k.levels), dp(k.prev_depth, k.levels);
+        CK(df_icp_estimate_depth(dc.ptr, nc.ptr, dp.ptr, np.ptr, vc.cols, vc.rows, dc.pitch, nc.pitch, k.levels, p.icp_iter_num, p.intr,
+                                 p.icp_dist_thres, p.icp_angle_thres, k.icp_T, k.icp_ok, k.icp_scratch, s));
+    } else if (color_tracked(k)) {
+        // DF_KINFU_COLOR_TRACKING: the model's intensity maps at the previous vertex maps, seen from poses.back(), then the ICP with
+        // the photometric rows
+        float cam2vol[12];
+        cam2vol_of(k, latest_pose(k), cam2vol);
+        const Levels<float> ic(k.cur_int, k.levels), mo(k.model_int, k.levels);
+        CK(df_model_intensity(vol_of(k), k.color_vol, to_aff(cam2vol), k.levels, vc.cols, vc.rows, vp.ptr, vp.pitch, mo.ptr, mo.pitch, s));
+        ++k.launches;
+        CK(df_icp_estimate_color(vc.ptr, nc.ptr, vp.ptr, np.ptr, ic.ptr, ic.pitch, mo.ptr, mo.pitch, vc.cols, vc.rows, vc.pitch, k.levels,
+                                 p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres, DF_COLOR_TRACK_WEIGHT,
+                                 DF_COLOR_TRACK_MAX_RESIDUAL, k.icp_T, k.icp_ok, k.icp_scratch, s));
+    } else
+    CK(df_icp_estimate(vc.ptr, nc.ptr, vp.ptr, np.ptr, vc.cols, vc.rows, vc.pitch, k.levels, p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres,
+                       k.icp_T, k.icp_ok, k.icp_scratch, s));
+    for (int i = 0; i < k.levels; ++i) k.launches += 2 * p.icp_iter_num[i];
+    ++k.launches;
+    return 0;
+}
+
+// ---- DF_KINFU_RELOCALISE (rules in include/dfusion.h) ---------------------------------------------------------------------------------
+// the gate on the ICP result in icp_T / icp_ok against the level-0 maps (pts, nrm), and its copy home (T and ok ride in it)
+int launch_gate(KinFu &k, const Img &pts, const Img &nrm)
+{
+    const df_kinfu_params &p = k.p;
+    CK(df_icp_inliers((const float *)k.cur_pts[0].ptr, k.cur_pts[0].pitch, (const float *)k.cur_nrm[0].ptr, k.cur_nrm[0].pitch, (const float *)pts.ptr,
+                      pts.pitch, (const float *)nrm.ptr, nrm.pitch, p.cols, p.rows, p.intr, k.icp_T, k.icp_ok, p.icp_dist_thres, p.icp_angle_thres,
+                      k.gate, k.gate_ws, k.stream));
+    ++k.launches;
+    CK(cudaMemcpyAsync(k.gate_host, k.gate, sizeof(df_reloc_gate), cudaMemcpyDeviceToHost, k.stream));
+    return 0;
+}
+
+// the match of the frame's code against the database; append: the harvest rule with the frame's accepted pose
+int launch_match(KinFu &k, int append, const float *pose)
+{
+    ++k.launches;
+    return df_fern_match(k.kf_codes, k.kf_poses, k.kf_count, DF_RELOC_KEYFRAMES, k.frame_code, DF_RELOC_FERNS, append, to_aff(pose), k.match,
+                         k.stream);
+}
+
+// a lost frame's keyframe candidates, in lookup order: the canonical volume ray-cast from the keyframe's pose into rl_pts / rl_nrm, the
+// geometric ICP against them, the gate.  accepted: one passed, and pose is its keyframe pose * T
+int try_keyframes(KinFu &k, float *pose, bool &accepted)
+{
+    const df_kinfu_params &p = k.p;
+    cudaStream_t s = k.stream;
+    CK(launch_match(k, 0, latest_pose(k)));
+    CK(cudaMemcpyAsync(k.match_host, k.match, sizeof(df_reloc_match), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    const df_reloc_match m = *k.match_host;
+    for (int c = 0; c < DF_RELOC_CANDIDATES && m.index[c] >= 0; ++c) {
+        const float *kf = m.pose[c];
+        CK(raycast_model(k, kf, k.rl_pts[0], k.rl_nrm[0]));
+        for (int i = 1; i < k.levels; ++i) {
+            CK(df_resize_points_normals((const float *)k.rl_pts[i - 1].ptr, k.rl_pts[i - 1].pitch, (const float *)k.rl_nrm[i - 1].ptr,
+                                        k.rl_nrm[i - 1].pitch, k.rl_pts[i - 1].cols, k.rl_pts[i - 1].rows, (float *)k.rl_pts[i].ptr,
+                                        k.rl_pts[i].pitch, (float *)k.rl_nrm[i].ptr, k.rl_nrm[i].pitch, s));
+            ++k.launches;
+        }
+        const Levels<float> vc(k.cur_pts, k.levels), nc(k.cur_nrm, k.levels), vp(k.rl_pts, k.levels), np(k.rl_nrm, k.levels);
+        CK(df_icp_estimate(vc.ptr, nc.ptr, vp.ptr, np.ptr, vc.cols, vc.rows, vc.pitch, k.levels, p.icp_iter_num, p.intr, p.icp_dist_thres,
+                           p.icp_angle_thres, k.icp_T, k.icp_ok, k.icp_scratch, s));
+        for (int i = 0; i < k.levels; ++i) k.launches += 2 * p.icp_iter_num[i];
+        ++k.launches;
+        CK(launch_gate(k, k.rl_pts[0], k.rl_nrm[0]));
+        CK(cudaStreamSynchronize(s));
+        k.last_ok = k.gate_host->ok;
+        if (!df_reloc_gate_accepts(k.gate_host)) continue;
+        dfh_aff_mul(kf, k.gate_host->T, pose);
+        accepted = true;
+        if (k.M > 0) {                                                 // the field's motion belonged to the lost trajectory
+            identity_transforms_kernel<<<div_up(k.M, 256), 256, 0, s>>>(k.M, k.nodes);
+            CK(cudaGetLastError());
+            ++k.launches;
+        }
+        k.lm_valid = false;
+        return 0;
+    }
+    return 0;
+}
+
+// the ICP and the gate; while lost, the keyframe candidates after it.  accepted = false: the frame is lost (nothing else changes)
+int track_reloc(KinFu &k, double &t_sync0, double &t_sync1, float *pose, bool &accepted)
+{
+    CK(launch_icp(k));                                                 // candidate 0: the ordinary ICP from the last good pose
+    CK(launch_gate(k, k.prev_pts[0], k.prev_nrm[0]));
+    t_sync0 = now_us();
+    CK(cudaStreamSynchronize(k.stream));
+    t_sync1 = now_us();
+    k.last_ok = k.gate_host->ok;
+    note_solve_overflow(k);
+    accepted = df_reloc_gate_accepts(k.gate_host) != 0;
+    if (accepted) dfh_aff_mul(latest_pose(k), k.gate_host->T, pose);
+    else if (k.lost) CK(try_keyframes(k, pose, accepted));
+    if (!accepted) {
+        if (!k.lost) {
+            const df_reloc_gate &g = *k.gate_host;
+            fprintf(stderr, "df_kinfu: tracking lost at frame %d (ICP ok %d, %d of %d pixels associated, RMS %.4f m); the model is kept and the "
+                            "camera relocalised from keyframes\n", k.frame_counter, g.ok, g.n_in, g.n_valid, g.n_in ? sqrt(g.sum_sq / g.n_in) : 0.0);
+        }
+        k.lost = true;
+        ++k.lost_frames;
+        return 0;
+    }
+    if (k.lost) { k.lost = false; ++k.relocalisations; }
+    return 0;
+}
+
+// Appends the frame's pose.  ICP failure resets the object (kinfu.cpp:276-277), which leaves frame_counter at 0; under DF_KINFU_RELOCALISE
+// it leaves accepted false instead and changes nothing.
+int track(KinFu &k, double &t_sync0, double &t_sync1, bool &accepted)
+{
+    cudaStream_t s = k.stream;
     float pose[12];
+    accepted = true;
     if (k.has_ov_pose) {               // lock-step parity hook: the caller's pose instead of this frame's ICP
         k.last_ok = 1;
         CK(cudaStreamSynchronize(s));
         note_solve_overflow(k);
         memcpy(pose, k.ov_pose, sizeof pose);
         k.has_ov_pose = false;
+        if (k.lost) { k.lost = false; ++k.relocalisations; }           // the caller's pose ends a loss as an accepted one does
+    } else if (reloc_on(k)) {
+        CK(track_reloc(k, t_sync0, t_sync1, pose, accepted));
+        if (!accepted) return 0;
     } else {
-        const Levels<float> vc(k.cur_pts, k.levels), nc(k.cur_nrm, k.levels), vp(k.prev_pts, k.levels), np(k.prev_nrm, k.levels);
-        if (p.flags & DF_KINFU_USE_DEPTH) {                            // estimateTransform(depth pyramids), kinfu.cpp:271
-            const Levels<unsigned short> dc(k.cur_depth, k.levels), dp(k.prev_depth, k.levels);
-            CK(df_icp_estimate_depth(dc.ptr, nc.ptr, dp.ptr, np.ptr, vc.cols, vc.rows, dc.pitch, nc.pitch, k.levels, p.icp_iter_num, p.intr,
-                                     p.icp_dist_thres, p.icp_angle_thres, k.icp_T, k.icp_ok, k.icp_scratch, s));
-        } else if (color_tracked(k)) {
-            // DF_KINFU_COLOR_TRACKING: the model's intensity maps at the previous vertex maps, seen from poses.back(), then the ICP with
-            // the photometric rows
-            float cam2vol[12];
-            cam2vol_of(k, latest_pose(k), cam2vol);
-            const Levels<float> ic(k.cur_int, k.levels), mo(k.model_int, k.levels);
-            CK(df_model_intensity(vol_of(k), k.color_vol, to_aff(cam2vol), k.levels, vc.cols, vc.rows, vp.ptr, vp.pitch, mo.ptr, mo.pitch, s));
-            ++k.launches;
-            CK(df_icp_estimate_color(vc.ptr, nc.ptr, vp.ptr, np.ptr, ic.ptr, ic.pitch, mo.ptr, mo.pitch, vc.cols, vc.rows, vc.pitch, k.levels,
-                                     p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres, DF_COLOR_TRACK_WEIGHT,
-                                     DF_COLOR_TRACK_MAX_RESIDUAL, k.icp_T, k.icp_ok, k.icp_scratch, s));
-        } else
-        CK(df_icp_estimate(vc.ptr, nc.ptr, vp.ptr, np.ptr, vc.cols, vc.rows, vc.pitch, k.levels, p.icp_iter_num, p.intr, p.icp_dist_thres, p.icp_angle_thres,
-                           k.icp_T, k.icp_ok, k.icp_scratch, s));
-        for (int i = 0; i < k.levels; ++i) k.launches += 2 * p.icp_iter_num[i];
-        ++k.launches;
+        CK(launch_icp(k));
         CK(cudaMemcpyAsync(k.pinned, k.icp_T, 12 * sizeof(float), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(k.pinned + 12, k.icp_ok, sizeof(int), cudaMemcpyDeviceToHost, s));
         t_sync0 = now_us();
@@ -360,6 +482,7 @@ int track(KinFu &k, double &t_sync0, double &t_sync1)
         if (!ok) return do_reset(k);                                  // kinfu.cpp:276-277
         dfh_aff_mul(latest_pose(k), k.pinned, pose);                 // poses_.back() * affine, kinfu.cpp:280
     }
+    if (reloc_on(k)) CK(launch_match(k, 1, pose));                     // the harvest
     mark(k, 2);
     k.poses.insert(k.poses.end(), pose, pose + 12);
     return 0;
@@ -612,8 +735,13 @@ int process(KinFu &k, const uint16_t *depth_dev, size_t depth_pitch, bool &fused
     begin_frame(k);
     if (k.has_depth_lens) CK(undistort_frame(k, depth_dev, depth_pitch));
     CK(preprocess(k, depth_dev, depth_pitch));
-    if (k.frame_counter == 0) return first_frame(k);
-    CK(track(k, t_sync0, t_sync1));
+    if (k.frame_counter == 0) {
+        CK(first_frame(k));
+        return reloc_on(k) ? launch_match(k, 1, latest_pose(k)) : 0;   // the first frame is keyframe 0
+    }
+    bool accepted;
+    CK(track(k, t_sync0, t_sync1, accepted));
+    if (!accepted) return 0;                                           // DF_KINFU_RELOCALISE: a lost frame
     if (k.frame_counter == 0) return 0;                                // tracking lost: the object was reset
     CK(dynamicfusion(k, k.cur_depth[0], k.cur_pts[0], &k.poses[k.poses.size() - 24]));
     CK(raycast_next(k));
@@ -691,7 +819,7 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         static const struct { const char *name; int flag; } env_flags[] = {
             {"DF_KINFU_WARPED_INTEGRATE", DF_KINFU_WARPED_INTEGRATE}, {"DF_KINFU_EXTEND_FIELD", DF_KINFU_EXTEND_FIELD},
             {"DF_KINFU_USE_DEPTH", DF_KINFU_USE_DEPTH}, {"DF_KINFU_F2_SOLVE", DF_KINFU_F2_SOLVE}, {"DF_KINFU_LIVE_MODEL", DF_KINFU_LIVE_MODEL},
-            {"DF_KINFU_COLOR", DF_KINFU_COLOR}};
+            {"DF_KINFU_COLOR", DF_KINFU_COLOR}, {"DF_KINFU_RELOCALISE", DF_KINFU_RELOCALISE}};
         for (const auto &f : env_flags) {
             const char *e = getenv(f.name);
             if (e && atoi(e) != 0) k->p.flags |= f.flag;
@@ -733,6 +861,18 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
         }
     }
     k->levels = used_levels(p);
+    if (p.flags & DF_KINFU_RELOCALISE) {
+        const char *why = (p.flags & DF_KINFU_USE_DEPTH) ? "cannot be combined with DF_KINFU_USE_DEPTH: its ICP reference is the model's depth pyramid"
+                          : (p.flags & DF_KINFU_LIVE_MODEL) ? "cannot be combined with DF_KINFU_LIVE_MODEL: its ICP reference is a raster of the live mesh, "
+                                                               "not a ray-cast of the canonical volume a keyframe can be seen in"
+                          : k->levels < 3 ? "needs at least 3 used ICP levels: the fern codes read the pyramid's level 2"
+                          : nullptr;
+        if (why) {
+            fprintf(stderr, "df_kinfu_create: DF_KINFU_RELOCALISE %s\n", why);
+            delete k;
+            return nullptr;
+        }
+    }
     k->max_nodes_cap = node_capacity(p);
     memcpy(k->vol_pose, p.volume_pose.R, 36); memcpy(k->vol_pose + 9, p.volume_pose.t, 12);
     dfh_mat3_inv(k->vol_pose, k->Rinv_vol);
@@ -780,6 +920,19 @@ extern "C" void *df_kinfu_create(const df_kinfu_params *pp)
     k->activity_bytes = df_volume_activity_bytes(v);
     ok = ok && k->activity.alloc(k->activity_bytes) == cudaSuccess && cudaMemset(k->activity, 0, k->activity_bytes) == cudaSuccess;
     ok = ok && k->project_ws.alloc(df_project_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
+    if (p.flags & DF_KINFU_RELOCALISE) {
+        std::vector<int32_t> table((size_t)DF_RELOC_FERNS * 12);
+        ok = ok && df_reloc_fern_table(DF_RELOC_SEED, k->cur_depth[2].cols, k->cur_depth[2].rows, DF_RELOC_FERNS, table.data()) == 0;
+        ok = ok && k->fern_table.alloc(table.size() * 4) == cudaSuccess &&
+             cudaMemcpy(k->fern_table, table.data(), table.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess;
+        ok = ok && k->frame_code.alloc(DF_RELOC_FERNS) == cudaSuccess && k->kf_codes.alloc((size_t)DF_RELOC_KEYFRAMES * DF_RELOC_FERNS) == cudaSuccess &&
+             k->kf_poses.alloc((size_t)DF_RELOC_KEYFRAMES * 48) == cudaSuccess && k->kf_count.alloc(64) == cudaSuccess;
+        ok = ok && k->gate_ws.alloc(DF_RELOC_GATE_WS_BYTES) == cudaSuccess && cudaMemset(k->gate_ws, 0, DF_RELOC_GATE_WS_BYTES) == cudaSuccess;
+        ok = ok && k->gate.alloc(sizeof(df_reloc_gate)) == cudaSuccess && k->match.alloc(sizeof(df_reloc_match)) == cudaSuccess;
+        ok = ok && cudaMallocHost(&k->gate_host, sizeof(df_reloc_gate)) == cudaSuccess && cudaMallocHost(&k->match_host, sizeof(df_reloc_match)) == cudaSuccess;
+        for (int l = 0, c = p.cols, r = p.rows; l < k->levels && ok; ++l, c /= 2, r /= 2)
+            ok = alloc_img(k->rl_pts[l], r, c, 16) == 0 && alloc_img(k->rl_nrm[l], r, c, 16) == 0;
+    }
     ok = ok && cudaMemset(k->project_ws, 0, df_project_workspace_bytes(p.cols, p.rows)) == cudaSuccess;
     ok = ok && cudaMemset(k->solve_stats, 0, 64) == cudaSuccess && cudaMemset(k->cloud_count, 0, 64) == cudaSuccess;
     ok = ok && cudaMallocHost(&k->pinned, 64) == cudaSuccess && (memset(k->pinned, 0, 64), true) && k->n_upd.alloc(64) == cudaSuccess && cudaMemset(k->n_upd, 0, 64) == cudaSuccess;
@@ -1020,9 +1173,31 @@ extern "C" int df_kinfu_get_info(void *h, long long *info, int n)
     cudaStreamSynchronize(k->stream);
     const unsigned long long nu = nu2[0];
     note_solve_overflow(*k);
-    const long long vals[13] = {k->frame_counter, k->M, k->last_cloud, (long long)(k->poses.size() / 12), k->last_ok, k->launches, k->resets,
-                                (long long)st[2], (long long)nu, (long long)st[4], (long long)nu2[1], k->solve_overflows, k->lm_fallbacks};
-    for (int i = 0; i < n && i < 13; ++i) info[i] = vals[i];
+    int keyframes = 0;
+    if (reloc_on(*k) && n > 16) {
+        cudaMemcpyAsync(&keyframes, k->kf_count, sizeof(int), cudaMemcpyDeviceToHost, k->stream);
+        cudaStreamSynchronize(k->stream);
+    }
+    const long long vals[17] = {k->frame_counter, k->M, k->last_cloud, (long long)(k->poses.size() / 12), k->last_ok, k->launches, k->resets,
+                                (long long)st[2], (long long)nu, (long long)st[4], (long long)nu2[1], k->solve_overflows, k->lm_fallbacks,
+                                k->lost, k->lost_frames, k->relocalisations, keyframes};
+    for (int i = 0; i < n && i < 17; ++i) info[i] = vals[i];
+    return 0;
+}
+
+extern "C" int df_kinfu_get_keyframes(void *h, float *poses_host, uint8_t *codes_host, int capacity, int *n)
+{
+    KinFu *k = (KinFu *)h;
+    if (!k || !reloc_on(*k) || !n) return (int)cudaErrorInvalidValue;
+    cudaSetDevice(k->device);
+    int count = 0;
+    CK(cudaMemcpyAsync(&count, k->kf_count, sizeof(int), cudaMemcpyDeviceToHost, k->stream));
+    CK(cudaStreamSynchronize(k->stream));
+    *n = count;
+    const int m = count < capacity ? count : capacity;
+    if (m <= 0) return 0;
+    if (poses_host) CK(cudaMemcpy(poses_host, k->kf_poses, (size_t)m * 48, cudaMemcpyDeviceToHost));
+    if (codes_host) CK(cudaMemcpy(codes_host, k->kf_codes, (size_t)m * DF_RELOC_FERNS, cudaMemcpyDeviceToHost));
     return 0;
 }
 

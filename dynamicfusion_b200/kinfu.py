@@ -26,6 +26,7 @@ COLOR = 256               # DF_KINFU_COLOR: fuse RGB-D frames into a colour volu
 LIVE_MODEL = 128          # DF_KINFU_LIVE_MODEL: ICP and the data term's association against the rendered live model, not the canonical ray-casts
 COLOR_TRACKING = 512      # DF_KINFU_COLOR_TRACKING: colour frames are tracked with photometric ICP rows as well (needs COLOR)
 WARPED_COLOR = 1024       # DF_KINFU_WARPED_COLOR: colour fused during per-voxel warped fusion (needs COLOR and WARPED_INTEGRATE)
+RELOCALISE = 2048         # DF_KINFU_RELOCALISE: keep the model through tracking loss and relocalise from fern-coded keyframes
 
 
 class KinFuParams:
@@ -148,11 +149,22 @@ class KinFu:
         return a[:9].reshape(3, 3), a[9:]
 
     def info(self) -> dict:
-        v = (C.c_longlong * 13)()
-        self.lib.df_kinfu_get_info(self.h, v, 13)
+        """df_kinfu_get_info; "lost", "lost_frames", "relocalisations" and "keyframes" are 0 on objects created without RELOCALISE"""
         keys = ["frame_counter", "nodes", "cloud_points", "poses", "icp_ok", "launches", "resets", "lm_iters", "n_updated", "pcg_iters",
-                "n_warped", "solve_overflows", "live_model_fallbacks"]
+                "n_warped", "solve_overflows", "live_model_fallbacks", "lost", "lost_frames", "relocalisations", "keyframes"]
+        v = (C.c_longlong * len(keys))()
+        self.lib.df_kinfu_get_info(self.h, v, len(keys))
         return dict(zip(keys, [int(x) for x in v]))
+
+    def keyframes(self):
+        """df_kinfu_get_keyframes: (poses [N, 12] float32 as getCameraPose's R row-major then t, fern codes [N, capi.RELOC_FERNS] uint8) of
+        the relocaliser's database.  Objects created with RELOCALISE only."""
+        n = C.c_int()
+        capi.check(self.lib.df_kinfu_get_keyframes(self.h, None, None, 0, C.byref(n)))
+        poses = np.empty((n.value, 12), np.float32)
+        codes = np.empty((n.value, capi.RELOC_FERNS), np.uint8)
+        capi.check(self.lib.df_kinfu_get_keyframes(self.h, poses.ctypes.data, codes.ctypes.data, n.value, C.byref(n)))
+        return poses, codes
 
     def set_overrides(self, bilateral_depth=None, pose=None, nodes=None) -> None:
         """df_kinfu_set_overrides (lock-step parity hook): numpy u16 [rows, cols] / (R 3x3, t 3) / float32 [M, 12] for the next frame"""

@@ -546,6 +546,97 @@ int df_icp_estimate_color(const float *const *vcurr, const float *const *ncurr, 
                           const int *cols, const int *rows, const size_t *pitch, int levels, const int *iters, df_intr intr, float dist_thres,
                           float angle_thres, float weight, float max_residual, float *T_dev, int *ok_dev, double *scratch, void *stream);
 
+/* ---- relocaliser (DF_KINFU_RELOCALISE): fern codes of the frame's depth, a keyframe database, and the gate on an ICP result ----------------
+ * Rules (tests/reloc_oracle.c states them again, independently; everything but the gate's residual sum is integer, so the kernels and the
+ * oracle agree bit for bit):
+ *   Table     DF_RELOC_FERNS ferns x 4 binary tests (u, v, theta_mm), drawn for a cols x rows image from the splitmix64 sequence of `seed`:
+ *             s = seed; next() = { s += 0x9e3779b97f4a7c15; z = s; z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9;
+ *             z = (z ^ (z >> 27)) * 0x94d049bb133111eb; return z ^ (z >> 31) } (u64 arithmetic).  For fern f = 0.., test j = 0..3 in
+ *             order: u = next() % cols, v = next() % rows, theta = DF_RELOC_NEAR_MM + next() % (DF_RELOC_FAR_MM - DF_RELOC_NEAR_MM).
+ *             df_reloc_fern_table writes them as int32 (u, v, theta) triples, fern-major: 12 * DF_RELOC_FERNS values.
+ *   Image     the frame loop codes the ICP pyramid's level 2 of the current depth (bilateral-filtered, truncated when
+ *             icp_truncate_depth_dist is set, halved twice by df_pyr_down: 160 x 120 for 640 x 480), with the table drawn for its size
+ *             and seed DF_RELOC_SEED.
+ *   Code      bit j of fern f is d(u, v) != 0 && d(u, v) < theta (u16 millimetres); the fern's byte is sum of bit_j << j.  A frame's code
+ *             is DF_RELOC_FERNS bytes.
+ *   Dissimilarity   of two codes: the number of ferns whose bytes differ.
+ *   Lookup    the DF_RELOC_CANDIDATES keyframes with the smallest dissimilarity to the frame, ranked by (dissimilarity, index).
+ *   Harvest   a frame whose pose the loop accepted (the first frame after create or reset, or a frame that passed the gate) is appended
+ *             with that pose when the database is empty, or when its smallest dissimilarity to the database is greater than
+ *             DF_RELOC_HARVEST_FERNS and the database holds fewer than DF_RELOC_KEYFRAMES entries.  A full database stops growing; nothing
+ *             is evicted.
+ *   Gate      for a pose increment T (the ICP's curr -> prev): at level 0, n_valid = current pixels whose vertex is not NaN, n_in = those the
+ *             ICP's association accepts (its projection, distance and angle tests, df_icp_accumulate's rule with dist_thres and
+ *             angle_thres), sum_sq = the sum over them of r * r in double, r = the row's float residual n_prev . (d - T v_curr).  The pose
+ *             is accepted when the ICP's ok holds, n_valid >= DF_RELOC_MIN_VALID, n_in >= DF_RELOC_MIN_INLIER_FRAC * n_valid (in float)
+ *             and sqrt(sum_sq / n_in) <= DF_RELOC_MAX_RMS.
+ *   Loss      a frame the gate rejects is lost: it fuses and extracts nothing, appends no pose, leaves the frame counter, the previous-frame
+ *             maps, the nodes, the cloud and both volumes as they were, and returns 0.  The object stays lost until a frame is accepted
+ *             or it is reset.
+ *   Relocalise  a frame that arrives while lost tries, in order: the ordinary ICP (with colour rows where the loop uses them) against the
+ *             kept previous-frame maps from the last good pose; then each lookup candidate: the canonical volume ray-cast from the
+ *             keyframe's pose into maps of the object's own (the kept maps stay as they were) and the geometric ICP against them, pose =
+ *             keyframe pose * T.  The first that passes the gate is the frame's pose and the frame continues as a tracked one.  A keyframe
+ *             win sets every node's transform to the identity (positions and weights kept); the ordinary ICP's win keeps the field.
+ *
+ * DF_RELOC_NEAR_MM / DF_RELOC_FAR_MM: the depth range the thresholds are drawn from, the working range of a structured-light or
+ * time-of-flight sensor at arm's length; a threshold outside the scene's depths makes a test that never changes.
+ * DF_RELOC_HARVEST_FERNS: a view becomes a keyframe when more than this many of its ferns differ from every stored one (Glocker et al. use
+ * a fifth of the ferns as the novelty bar; here a smaller share, so that a slow sweep of one scene still leaves several keyframes).
+ * DF_RELOC_MIN_VALID, DF_RELOC_MIN_INLIER_FRAC and DF_RELOC_MAX_RMS: a frame with almost no depth, or whose points mostly find no model
+ * surface, or whose associated points lie centimetres off it, is not tracked.  The inlier share is of every valid pixel, and a volume
+ * smaller than the view leaves the pixels beyond it unassociated: with the 1 m cube of the synthetic sequences some 45 % of a 640 x 480
+ * frame sees no model, and the warped loop with a growing field was measured at 20 % on a tracked frame of C2 (frame 53), hence 0.1;
+ * blank frames and views of another scene associate next to nothing.  The RMS bar allows the breathing surfaces of the non-rigid loop, whose ray-cast reference is the
+ * undeformed canonical model. */
+#define DF_RELOC_FERNS 500
+#define DF_RELOC_CANDIDATES 3
+#define DF_RELOC_KEYFRAMES 512
+#define DF_RELOC_NEAR_MM 400
+#define DF_RELOC_FAR_MM 3000
+#define DF_RELOC_SEED 0x5eedf00dull
+#define DF_RELOC_HARVEST_FERNS 40
+#define DF_RELOC_MIN_VALID 5000
+#define DF_RELOC_MIN_INLIER_FRAC 0.1f
+#define DF_RELOC_MAX_RMS 0.03f
+
+/* the gate's result as df_icp_inliers writes it (72 bytes): the ICP's T and ok copied alongside the counts, so that one copy brings all of
+ * it to the host */
+typedef struct df_reloc_gate {
+    float T[12];
+    int ok, n_valid, n_in, pad;
+    double sum_sq;
+} df_reloc_gate;
+
+/* df_fern_match's output (device): the lookup's candidates (index -1 and dissimilarity DF_RELOC_FERNS + 1 past the database's count), whether
+ * the frame was appended, the database's count after the call, and the candidates' poses (12 floats each, zero past the count) */
+typedef struct df_reloc_match {
+    int index[DF_RELOC_CANDIDATES];
+    int dissimilarity[DF_RELOC_CANDIDATES];
+    int appended, count;
+    float pose[DF_RELOC_CANDIDATES][12];
+} df_reloc_match;
+
+/* the Table rule for a cols x rows image into out_host (12 * n_ferns int32); host only.  cols, rows or n_ferns < 1: cudaErrorInvalidValue */
+int df_reloc_fern_table(unsigned long long seed, int cols, int rows, int n_ferns, int32_t *out_host);
+/* the Code rule: one thread per fern, one launch.  depth: device u16, pitch in bytes (even, at least cols * 2); table: device, as
+ * df_reloc_fern_table writes it for this size (a test outside the image reads as 0 bit); codes: device, n_ferns bytes. */
+int df_fern_encode(const uint16_t *depth, size_t pitch, int cols, int rows, const int32_t *table, int n_ferns, uint8_t *codes, void *stream);
+/* Dissimilarity, Lookup and (append != 0) the Harvest rule in one single-block launch.  db_codes: device, capacity x n_ferns bytes;
+ * db_poses: device, capacity x 12 floats; count: device int, the entries held (updated on an append); code: device, the frame's n_ferns bytes;
+ * pose: the frame's pose, stored on an append.  capacity <= DF_RELOC_KEYFRAMES, n_ferns <= DF_RELOC_FERNS, else cudaErrorInvalidValue. */
+int df_fern_match(uint8_t *db_codes, float *db_poses, int *count, int capacity, const uint8_t *code, int n_ferns, int append, df_aff3f pose,
+                  df_reloc_match *out, void *stream);
+/* the Gate rule's counts at one level: vertex and normal maps as df_icp_accumulate's (float4, pitches in bytes, multiples of 16), T_dev
+ * (device, 12 floats; NULL: the identity) and ok_dev (device int; NULL: 1) copied into out.  One launch; the residual sum is reduced in a
+ * fixed order (run-to-run deterministic).  ws: device, DF_RELOC_GATE_WS_BYTES, zeroed before its first use (every call leaves it zeroed). */
+#define DF_RELOC_GATE_WS_BYTES 4096
+int df_icp_inliers(const float *vcurr, size_t vcurr_pitch, const float *ncurr, size_t ncurr_pitch, const float *vprev, size_t vprev_pitch,
+                   const float *nprev, size_t nprev_pitch, int cols, int rows, df_intr intr, const float *T_dev, const int *ok_dev,
+                   float dist_thres, float angle_thres, df_reloc_gate *out, void *ws, void *stream);
+/* the Gate rule's decision on a result of df_icp_inliers; host only */
+int df_reloc_gate_accepts(const df_reloc_gate *g);
+
 /* ------------------------------------------------------------------ warp field ------------------------------------------------------------ */
 /* deformation_node (warp_field.hpp:35-40) as 12 floats: vertex[3], rotation quat (w,x,y,z), dual/translation quat
  * (w,x,y,z) = 0.5*t*r (dual_quaternion.hpp:59-63), weight. */
@@ -768,6 +859,18 @@ typedef struct df_kinfu_params {
                                       run with DF_KINFU_WARPED_INTEGRATE alone, bit for bit.  Snapshots carry the flag in their parameters.
                                       Environment: DF_KINFU_WARPED_COLOR=1 adds it to every object that has both other flags; others are left as they
                                       are. */
+#define DF_KINFU_RELOCALISE 2048    /* keep the model through tracking loss and relocalise the camera from fern-coded keyframes (rules below, "relocaliser")
+                                      instead of resetting when the ICP fails.  Every frame's level-2 depth is fern-coded (df_fern_encode) and every
+                                      ICP result goes through the gate (df_icp_inliers); a frame that fails it is lost: it returns 0 and changes no
+                                      state.  Frames that arrive while lost try the ordinary ICP from the last good pose first, then the
+                                      DF_RELOC_CANDIDATES most similar keyframes.  A tracked frame launches three kernels more (encode, gate, match);
+                                      its {T, ok} and the gate's counts come home in one copy, at the ICP's existing synchronisation.  Combines with
+                                      every flag but DF_KINFU_USE_DEPTH and DF_KINFU_LIVE_MODEL (refused at create, reason on stderr: their ICP
+                                      references are depth pyramids and a raster of the live mesh, not ray-casts of the canonical volume); needs at
+                                      least 3 used ICP levels.  The pose of df_kinfu_set_overrides bypasses the gate.  df_kinfu_get_info[13..16]
+                                      report it; df_kinfu_reset empties the keyframe database and ends a loss; snapshots carry both (version 5).
+                                      The C++ mirror takes it in dfusion_flags (KinFu::isLost()).  Without the flag nothing is computed,
+                                      allocated or launched, and ICP failure resets the object as before.  Environment: DF_KINFU_RELOCALISE=1. */
 
 /* which = 0: KinFuParams::default_params_dynamicfusion (kinfu.cpp:14-49); 1: default_params (kinfu.cpp:55-89) */
 void df_kinfu_default_params(df_kinfu_params *p, int which);
@@ -778,7 +881,7 @@ int df_kinfu_set_stream(void *kinfu, void *stream);
 /* KinFu::reset (kinfu.cpp:196-207) */
 int df_kinfu_reset(void *kinfu);
 /* KinFu::operator()(depth) (kinfu.cpp:221-305).  Returns 1 = frame fused and ray-cast image available, 0 = first frame or
- * tracking reset (the reference's `false`), < 0 = -(cudaError).  _host: depth is a HOST u16 image (any pitch), copied to
+ * tracking reset (the reference's `false`; under DF_KINFU_RELOCALISE a lost frame instead), < 0 = -(cudaError).  _host: depth is a HOST u16 image (any pitch), copied to
  * the device inside the call (the path apps/demo.cpp takes: imread -> upload -> operator()); _device: depth already in HBM. */
 int df_kinfu_process_host(void *kinfu, const uint16_t *depth_host, size_t pitch);
 int df_kinfu_process_device(void *kinfu, const uint16_t *depth_dev, size_t pitch);
@@ -835,8 +938,15 @@ int df_kinfu_get_pose(void *kinfu, int time, float *pose12_host);
  * [8] voxels written by the last integrate (DF_KINFU_STAGE_TIMING only), [9] solver PCG iterations (last frame),
  * [10] voxels carried through the warp field by the last df_integrate_warped (DF_KINFU_WARPED_INTEGRATE + STAGE_TIMING),
  * [11] frames whose warp solve was skipped because a normal-matrix row overflowed (df_solve_data_term: stats[5]); also reported on stderr,
- * [12] DF_KINFU_LIVE_MODEL: frames that fell back to the ray-casts because the live mesh could not be built (the first one reported on stderr) */
+ * [12] DF_KINFU_LIVE_MODEL: frames that fell back to the ray-casts because the live mesh could not be built (the first one reported on stderr),
+ * DF_KINFU_RELOCALISE (0 without it): [13] 1 while tracking is lost, [14] lost frames so far, [15] relocalisations so far (a loss that
+ * ended), [16] keyframes held.  A tracked frame's launch count [5] includes df_fern_encode, df_icp_inliers and df_fern_match.  Counters [14]
+ * and [15] count over the object's life, as [6] does. */
 int df_kinfu_get_info(void *kinfu, long long *info_host, int n);
+/* DF_KINFU_RELOCALISE: the keyframe database -- *n = the entries held; the first min(*n, capacity) poses (12 floats each, as
+ * df_kinfu_get_pose) into poses_host and codes (DF_RELOC_FERNS bytes each) into codes_host (either may be NULL).  An object without the
+ * flag: cudaErrorInvalidValue.  Synchronous. */
+int df_kinfu_get_keyframes(void *kinfu, float *poses_host, uint8_t *codes_host, int capacity, int *n);
 /* device buffers of the current state, the `which` of df_kinfu_get_buffer / _read_buffer */
 #define DF_KINFU_BUF_VOLUME 0              /* the TSDF volume (u32) */
 #define DF_KINFU_BUF_DISTS 1
@@ -919,6 +1029,13 @@ int df_kinfu_get_stage_ms(void *kinfu, float *ms_host, int n);
  * Whether a version-4 snapshot of a colour object holds the camera record follows from its length (72 bytes).  A present record passes
  * df_lens_check and is not the zero lens; at least one is present; a colour lens needs the camera record.  A load also requires the
  * object's lenses to equal the records byte for byte (no record: no lens set).
+ * Version 5 is what an object with DF_KINFU_RELOCALISE writes (without the flag it writes version 1 to 4, byte for byte as above): the
+ * content of the version its flags, camera and lenses give, with u32 version = 5, followed by
+ *   relocaliser u32 base version (the 1 to 4 the content has), u8 lost, 3 zero bytes, i64 lost frames, i64 relocalisations, u64 fern seed
+ *               (DF_RELOC_SEED), i32 keyframe count, i32 ferns (DF_RELOC_FERNS); count x DF_RELOC_FERNS code bytes; count x 12 pose floats;
+ *               u64 the section's length, these 8 bytes included (so a reader finds the section from the end)
+ * The last good pose is the pose chain's last entry.  Version 5 must match the flag of the stored params both ways; a section that is
+ * truncated, has another seed or fern count, more keyframes than DF_RELOC_KEYFRAMES, or a length its count does not give is rejected.
  * The node grid is rebuilt on load.  Per-frame scratch is not stored: dists, the current-frame images and pyramids, the canonical maps,
  * the solver statistics and workspaces hold undefined contents after a load until the next frame writes them.
  *

@@ -43,6 +43,7 @@ namespace kfusion
         // reference's behaviour.  (The same switches exist as environment variables for an unchanged apps/demo.cpp, dfusion.h.)
         int dfusion_flags = 0;             // DF_KINFU_WARPED_INTEGRATE (8) | DF_KINFU_EXTEND_FIELD (16) | DF_KINFU_COLOR (256) | DF_KINFU_COLOR_TRACKING (512)
                                            // | DF_KINFU_WARPED_COLOR (1024: with COLOR and WARPED_INTEGRATE, colour fused through the warp field)
+                                           // | DF_KINFU_RELOCALISE (2048: keep the model through tracking loss, isLost())
         float fusion_weight_scale = 0.f;   // df_integrate_warped's weight quantisation (0: every sample weighs 1)
         float extend_radius = 0.f;         // df_extend_field's support radius in metres (0: 0.03)
     };
@@ -74,6 +75,9 @@ namespace kfusion
         // not in the reference: snapshots of the whole reconstruction (df_kinfu_save / df_kinfu_load, include/dfusion.h).  load() needs an
         // object made with the same parameters and resumes the sequence exactly where save() left it; both return false on failure
         // (I/O error, malformed file, other parameters, another colour camera), and a failed load leaves the object unchanged.
+        // not in the reference: tracking loss (dfusion_flags DF_KINFU_RELOCALISE, 2048): true while the last frame failed the relocaliser's gate;
+        // operator() then returned false and left the reconstruction as it was, and the camera is relocalised from keyframes by later frames
+        bool isLost() const;
         bool save(const std::string& path) const;
         bool load(const std::string& path);
         // not in the reference: the triangle mesh of the canonical model (live = true: carried into the current frame by the warp field),
